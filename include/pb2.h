@@ -1,5 +1,5 @@
 /*
- * pb2.h — C ABI of the B200-native pbrt-v3 path-tracing hot path.
+ * pb2.h — C ABI of the H100-native pbrt-v3 path-tracing hot path.
  *
  * pbrt-v3 has no dlopen plugin ABI: its "plugins" are C++ classes selected by name in
  * src/core/api.cpp.  The hot path sits behind these reference interfaces:

@@ -1,9 +1,9 @@
-"""pbrt_v3_b200 — B200-native path-tracing hot path behind pbrt-v3's plugin API.
+"""pbrt_v3_b200 — H100-native path-tracing hot path behind pbrt-v3's plugin API.
 
 Python is only the driver here (tests, bench.py, multi-GPU launch through torch.distributed):
 everything below is a thin ctypes view of
 
-* ``lib/libpb2.so`` — the C ABI of ``include/pb2.h`` (CUDA kernels, sm_100a) plus the C++ host-side
+* ``lib/libpb2.so`` — the C ABI of ``include/pb2.h`` (CUDA kernels, sm_90a) plus the C++ host-side
   scene front end (``csrc/host``: .pbrt parser, pbrt's Shape/Primitive/BVHAccel/Film/... classes,
   SAH BVH build), exported for scripting through the ``pb2h_*`` helpers of ``csrc/host/capi.cpp``.
 

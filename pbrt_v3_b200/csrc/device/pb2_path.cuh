@@ -154,7 +154,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
     }
     const float *distrib = (LAZY && lazyDistrib) ? lazyDistrib : lightDistLookup(sc.lightDist, isect.p);
     // The lane lives in HBM and is updated in place, the sampler's dimension counter included (a
-    // register copy of ln.smp across this function was measured: -12 %, the 128-register budget is full).
+    // register copy of ln.smp across this function would not fit: the 128-register budget is full).
     DSampler &smp = ln.smp;
 
     ln.doNEE = bsdf.nLobes > 0;

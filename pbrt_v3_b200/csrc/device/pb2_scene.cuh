@@ -213,9 +213,15 @@ PB2_HD bool slabTestT(float minx, float miny, float minz, float maxx, float maxy
     return !miss1 & !miss2 & (tMin < rayTMax) & (tMax > 0);
 }
 
+// Pairs of floats, lane 0 = child 0, lane 1 = child 1.  sm_90 has no packed FP32x2 add / multiply: each
+// pair is two IEEE operations, never contracted into an FMA.
+#if defined(__CUDA_ARCH__)
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+#endif
+
 // Both children of a two-child record at once.  On the device the subtractions, multiplications and
-// the far-plane scaling run as packed FP32x2 operations (FADD2 / FMUL2, sm_100: `__fadd2_rn`,
-// `__fmul2_rn`), lane 0 = child 0, lane 1 = child 1 - per component these are the IEEE operations of
+// the far-plane scaling run on pairs (fadd2 / fmul2) - per component these are the IEEE operations of
 // slabTestT, so the verdicts and tMin values are bit-identical to two slabTestT calls.
 PB2_HD void slabTestPair(float4 q0, float4 q1, float4 q2, const DRaySetup &r, float rayTMax, bool *pass0, bool *pass1,
                          float *tMin0, float *tMin1) {
@@ -229,12 +235,12 @@ PB2_HD void slabTestPair(float4 q0, float4 q1, float4 q2, const DRaySetup &r, fl
     const float2 nox = make_float2(-r.o.x, -r.o.x), noy = make_float2(-r.o.y, -r.o.y), noz = make_float2(-r.o.z, -r.o.z);
     const float2 ix = make_float2(r.invDir.x, r.invDir.x), iy = make_float2(r.invDir.y, r.invDir.y), iz = make_float2(r.invDir.z, r.invDir.z);
     const float2 sc2 = make_float2(kSlabScale, kSlabScale);
-    float2 tMin = __fmul2_rn(__fadd2_rn(nearX, nox), ix);
-    float2 tMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farX, nox), ix), sc2);
-    const float2 tyMin = __fmul2_rn(__fadd2_rn(nearY, noy), iy);
-    const float2 tyMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farY, noy), iy), sc2);
-    const float2 tzMin = __fmul2_rn(__fadd2_rn(nearZ, noz), iz);
-    const float2 tzMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farZ, noz), iz), sc2);
+    float2 tMin = fmul2(fadd2(nearX, nox), ix);
+    float2 tMax = fmul2(fmul2(fadd2(farX, nox), ix), sc2);
+    const float2 tyMin = fmul2(fadd2(nearY, noy), iy);
+    const float2 tyMax = fmul2(fmul2(fadd2(farY, noy), iy), sc2);
+    const float2 tzMin = fmul2(fadd2(nearZ, noz), iz);
+    const float2 tzMax = fmul2(fmul2(fadd2(farZ, noz), iz), sc2);
     {
         const bool miss1 = (tMin.x > tyMax.x) | (tyMin.x > tMax.x);
         float a = (tyMin.x > tMin.x) ? tyMin.x : tMin.x, b = (tyMax.x < tMax.x) ? tyMax.x : tMax.x;
@@ -265,7 +271,7 @@ PB2_HD void slabTestPair(float4 q0, float4 q1, float4 q2, const DRaySetup &r, fl
 // exactly the boxes where some entry parameter exceeds ANOTHER axis' exit parameter.  `tMin <= tMax` also compares the
 // two parameters of the same axis; they can only be out of order when the exit parameter is negative (the far-plane
 // scaling by 1 + 2 gamma(3) moves it away from zero), and then the reference's final `tMax > 0` rejects the box as well.
-// FMNMX3 takes three operands: a box costs 5 instructions after the multiplications instead of ~16.
+// Four min / max instructions per box after the multiplications instead of ~16 compare-and-selects.
 PB2_HD void slabTestPairFast(float4 q0, float4 q1, float4 q2, const DRaySetup &r, float rayTMax, bool *pass0, bool *pass1,
                              float *tMin0, float *tMin1) {
 #if defined(__CUDA_ARCH__)
@@ -277,12 +283,12 @@ PB2_HD void slabTestPairFast(float4 q0, float4 q1, float4 q2, const DRaySetup &r
     const float2 nox = make_float2(-r.o.x, -r.o.x), noy = make_float2(-r.o.y, -r.o.y), noz = make_float2(-r.o.z, -r.o.z);
     const float2 ix = make_float2(r.invDir.x, r.invDir.x), iy = make_float2(r.invDir.y, r.invDir.y), iz = make_float2(r.invDir.z, r.invDir.z);
     const float2 sc2 = make_float2(kSlabScale, kSlabScale);
-    const float2 tMin = __fmul2_rn(__fadd2_rn(nearX, nox), ix);
-    const float2 tMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farX, nox), ix), sc2);
-    const float2 tyMin = __fmul2_rn(__fadd2_rn(nearY, noy), iy);
-    const float2 tyMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farY, noy), iy), sc2);
-    const float2 tzMin = __fmul2_rn(__fadd2_rn(nearZ, noz), iz);
-    const float2 tzMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farZ, noz), iz), sc2);
+    const float2 tMin = fmul2(fadd2(nearX, nox), ix);
+    const float2 tMax = fmul2(fmul2(fadd2(farX, nox), ix), sc2);
+    const float2 tyMin = fmul2(fadd2(nearY, noy), iy);
+    const float2 tyMax = fmul2(fmul2(fadd2(farY, noy), iy), sc2);
+    const float2 tzMin = fmul2(fadd2(nearZ, noz), iz);
+    const float2 tzMax = fmul2(fmul2(fadd2(farZ, noz), iz), sc2);
     const float lo0 = fmaxf(fmaxf(tMin.x, tyMin.x), tzMin.x), hi0 = fminf(fminf(tMax.x, tyMax.x), tzMax.x);
     const float lo1 = fmaxf(fmaxf(tMin.y, tyMin.y), tzMin.y), hi1 = fminf(fminf(tMax.y, tyMax.y), tzMax.y);
     *tMin0 = lo0;
@@ -383,14 +389,11 @@ PB2_HD float4 ldg4(const float4 *p) {
 #endif
 }
 PB2_HD int asInt(float f) { return (int)floatBits(f); }
-// 32 bytes per lane in one request (LDG.E.256, sm_100): a node record is fetched with half as many L1 wavefronts as
-// with 16-byte loads - each lane of a warp reads another record, and the L1 data pipe serves such a scattered request
-// one lane per cycle whatever its width (ncu: l1tex__data_pipe_lsu_wavefronts at 88 % of peak with 16-byte loads).
+// 32 bytes of a node record.  sm_90's widest global load is 16 bytes per lane: two read-only 16-byte loads.
 #if defined(__CUDA_ARCH__)
 __device__ __forceinline__ void ldg256(const float4 *p, float4 &a, float4 &b) {
-    asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-        : "l"(p));
+    a = __ldg(p);
+    b = __ldg(p + 1);
 }
 #else
 inline void ldg256(const float4 *p, float4 &a, float4 &b) { a = p[0]; b = p[1]; }

@@ -125,12 +125,12 @@ PB2_HD void slabTestPair4(float4 a, float4 b, float4 c, const DRaySetup &r, floa
     const float2 nox = make_float2(-r.o.x, -r.o.x), noy = make_float2(-r.o.y, -r.o.y), noz = make_float2(-r.o.z, -r.o.z);
     const float2 ix = make_float2(r.invDir.x, r.invDir.x), iy = make_float2(r.invDir.y, r.invDir.y), iz = make_float2(r.invDir.z, r.invDir.z);
     const float2 sc2 = make_float2(kSlabScale, kSlabScale);
-    const float2 tMin = __fmul2_rn(__fadd2_rn(nearX, nox), ix);
-    const float2 tMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farX, nox), ix), sc2);
-    const float2 tyMin = __fmul2_rn(__fadd2_rn(nearY, noy), iy);
-    const float2 tyMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farY, noy), iy), sc2);
-    const float2 tzMin = __fmul2_rn(__fadd2_rn(nearZ, noz), iz);
-    const float2 tzMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farZ, noz), iz), sc2);
+    const float2 tMin = fmul2(fadd2(nearX, nox), ix);
+    const float2 tMax = fmul2(fmul2(fadd2(farX, nox), ix), sc2);
+    const float2 tyMin = fmul2(fadd2(nearY, noy), iy);
+    const float2 tyMax = fmul2(fmul2(fadd2(farY, noy), iy), sc2);
+    const float2 tzMin = fmul2(fadd2(nearZ, noz), iz);
+    const float2 tzMax = fmul2(fmul2(fadd2(farZ, noz), iz), sc2);
     {
         const bool miss1 = (tMin.x > tyMax.x) | (tyMin.x > tMax.x);
         float lo = (tyMin.x > tMin.x) ? tyMin.x : tMin.x, hi = (tyMax.x < tMax.x) ? tyMax.x : tMax.x;
@@ -167,12 +167,12 @@ PB2_HD void slabTestPair4Fast(float4 a, float4 b, float4 c, const DRaySetup &r, 
     const float2 nox = make_float2(-r.o.x, -r.o.x), noy = make_float2(-r.o.y, -r.o.y), noz = make_float2(-r.o.z, -r.o.z);
     const float2 ix = make_float2(r.invDir.x, r.invDir.x), iy = make_float2(r.invDir.y, r.invDir.y), iz = make_float2(r.invDir.z, r.invDir.z);
     const float2 sc2 = make_float2(kSlabScale, kSlabScale);
-    const float2 tMin = __fmul2_rn(__fadd2_rn(nearX, nox), ix);
-    const float2 tMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farX, nox), ix), sc2);
-    const float2 tyMin = __fmul2_rn(__fadd2_rn(nearY, noy), iy);
-    const float2 tyMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farY, noy), iy), sc2);
-    const float2 tzMin = __fmul2_rn(__fadd2_rn(nearZ, noz), iz);
-    const float2 tzMax = __fmul2_rn(__fmul2_rn(__fadd2_rn(farZ, noz), iz), sc2);
+    const float2 tMin = fmul2(fadd2(nearX, nox), ix);
+    const float2 tMax = fmul2(fmul2(fadd2(farX, nox), ix), sc2);
+    const float2 tyMin = fmul2(fadd2(nearY, noy), iy);
+    const float2 tyMax = fmul2(fmul2(fadd2(farY, noy), iy), sc2);
+    const float2 tzMin = fmul2(fadd2(nearZ, noz), iz);
+    const float2 tzMax = fmul2(fmul2(fadd2(farZ, noz), iz), sc2);
     const float lo0 = fmaxf(fmaxf(tMin.x, tyMin.x), tzMin.x), hi0 = fminf(fminf(tMax.x, tyMax.x), tzMax.x);
     const float lo1 = fmaxf(fmaxf(tMin.y, tyMin.y), tzMin.y), hi1 = fminf(fminf(tMax.y, tyMax.y), tzMax.y);
     *tMin0 = lo0;

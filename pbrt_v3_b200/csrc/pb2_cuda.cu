@@ -1,4 +1,4 @@
-// CUDA kernels and the C ABI (include/pb2.h) of the path-tracing hot path, sm_100a only.
+// CUDA kernels and the C ABI (include/pb2.h) of the path-tracing hot path, sm_90a only.
 //
 // Kernels
 //   k_build_leaf_records      scene upload: gather triangle vertices into BVH-ordered 48-B leaf records
@@ -412,9 +412,6 @@ struct pb2_scene {
     unsigned *wfHostCounts = nullptr;  // pinned
     int wfCapacity = 0;
     std::vector<cudaEvent_t> traceEvents;
-    int pipesChosen = 0;                     // wavefront pipelines for this scene, chosen from its second frame (0 = not yet)
-    int framesRendered = 0;
-    cudaEvent_t frameEvents[2] = {nullptr, nullptr};
     int2 *wfSpill = nullptr;                 // k_wf_trace_pool: stack entries beyond its shared-memory depth
     void *chainBuf = nullptr;                // device copies of {DScene, DRenderParams} for the CHAIN trace kernels
     cudaStream_t pipeStreams[4] = {nullptr, nullptr, nullptr, nullptr};   // streams of the wavefront pipelines 1.. (renderWavefront)
@@ -886,17 +883,17 @@ typedef void (*TraceKernel)(DScene, WfPool, int, WfChain);
 typedef void (*AdvanceKernel)(DScene, DRenderParams, WfPool, int, int, int, float4 *, unsigned long long *);
 
 // Which traversal kernel a scene is traced with (pb2_wavefront.cuh), and its launch shape.
-//   default                   k_wf_trace_w<2>: persistent warps over the two-child records, 32-byte loads
+//   default                   k_wf_trace_w<2>: persistent warps over the two-child records (a record is read as
+//                             pairs of 16-byte loads, ldg256)
 //   PB2_FLAG_WIDE4            k_wf_trace_w<4>: the same over the four-child records (two tree levels per fetch)
-//   PB2_FLAG_LD128            either of them with 16-byte instead of 32-byte loads
+//   PB2_FLAG_LD128            either of them with one 16-byte load per quarter record (on sm_90 the same loads)
 //   PB2_FLAG_LINEAR_NODES     k_wf_trace: the same over the reference's 32-B LinearBVHNode array; also the fallback for
 //                             scenes beyond the record limits (2^27 primitives, 16 per leaf)
 //   PB2_FLAG_PLAIN_TRACE /    k_wf_trace_plain: one thread per ray, BVHAccel::Intersect as written (the counting form
 //   PB2_FLAG_COUNT_TRAVERSAL  also returns node / primitive counters)
 //   PB2_FLAG_SMALL_STACK      4 instead of 16 shared-memory stack entries per lane (tests: forces the local-memory spill)
-// Measured (1920x1080x16, 1 M soup / instanced / killeroo-like, Msamples/s): two-child 207.4 / 173.4 / 187.3, four-child
-// 204.8 / 163.9 / 181.9 - the four-child visit needs as many instructions per box as the two-child one (ordering and up
-// to three deferred entries), so halving the dependent fetches buys nothing; 32-byte loads: +4 % on both.
+// The four-child visit needs as many instructions per box as the two-child one (ordering and up to three deferred
+// entries), so halving the dependent fetches need not pay; the two-child kernel is the default.
 struct TraceLaunch {
     TraceKernel fn = nullptr;
     int block = 128;
@@ -932,9 +929,7 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
         t.name = "k_wf_trace_pool";
         if (!scene->wfSpill)   // per pipeline: up to 8 resident blocks per SM x 4 warps x PL_R slots x PL_SPILL entries
             CUDA_TRY(cudaMalloc((void **)&scene->wfSpill, (size_t)kMaxPipes * g_numSMs * 8 * 4 * PL_R * PL_SPILL * sizeof(int2)));
-        // 48 rays per warp, 8 stack entries per ray in shared memory: 25 KB per block, 8 resident blocks per SM.  Sweep (1 M soup,
-        // 16 spp, one pipeline; k_wf_trace_w: 219.3 Msamples/s): 64 rays / 12 entries / 5 blocks 194.6; NSUB 2: 190.8; leaf steps
-        // from 16 ready rays: 192.9; NSUB 1: 178.9; this one 203.6; 40 rays: 202.2; 64 rays / 8 entries / 6 blocks: 196.3
+        // 48 rays per warp, 8 stack entries per ray in shared memory: 25 KB per block, 8 resident blocks per SM
         t.fn = k_wf_trace_pool<4, 8, 16, 12, 48, 8>;
         t.smem = 4 * sizeof(PoolWarp<48, 8>);
         CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)t.smem));
@@ -950,8 +945,7 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
             else t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 7, false, false, true> : k_wf_trace_w<4, 1, 8, 4, 16, 7, false, false, true>;
         }
     } else if (records) {
-        // LEAF_T = 1: a warp turns to its leaves as soon as one lane holds one (sweep 16 / 12 / 8 / 6 / 4 / 3 / 2 / 1 at
-        // 16 spp: 192.8 / 199.3 / 202.9 / 203.6 / 204.4 / 204.7 / 205.2 / 205.9 Msamples/s); 56 registers, 9 blocks / SM
+        // LEAF_T = 1: a warp turns to its leaves as soon as one lane holds one; 56 registers (room for 9 blocks / SM)
         t.name = "k_wf_trace_w<2>";
         if (flags & PB2_FLAG_LD128) {
             if (instanced) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true, true>;
@@ -961,10 +955,8 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
             if (instanced) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true, true, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true, true, true>;
             else if (spheres) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true, false, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true, false, true>;
             else if (flags & PB2_FLAG_LEAF_TMA) t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 5, false, false, true, true>;
-            // (round-2 sweep around these parameters with the min/max slab tests and 32-byte loads in place - LEAF_T 2 / 4, NSUB 3 / 6,
-            // FETCH_T 12, 10 resident blocks: 221.6 ... 223.2 against 224.0 Msamples/s at 16 spp; the scheduling constants are flat)
             else t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 9, false, false, true> : k_wf_trace_w<2, 1, 8, 4, 16, 9, false, false, true>;
-            // (experiment, PB2_FLAG_CHAIN; measured and NOT adopted, DESIGN.md section 3) the default kernels with the light step
+            // (experiment, PB2_FLAG_CHAIN; not the default, DESIGN.md section 3) the default kernels with the light step
             // inside: shadow ray -> MIS ray -> continuation follow each other in the lane, one round per bounce
             if (wantChain && !small && !(flags & PB2_FLAG_LEAF_TMA)) {
                 t.chain = true;
@@ -987,6 +979,8 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
     }
     int blocksPerSM = 1;
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocksPerSM, t.fn, t.block, t.smem));
+    // the persistent grid: at most 8 blocks per SM (the pool kernel's spill buffer is sized for 8)
+    blocksPerSM = std::max(1, std::min(blocksPerSM, 8));
     // ask for exactly the shared-memory carve-out the resident blocks need; the rest stays L1
     cudaFuncAttributes fa;
     CUDA_TRY(cudaFuncGetAttributes(&fa, t.fn));
@@ -997,7 +991,7 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
     if (verbose)
         fprintf(stderr, "pb2: trace kernel %s: %d regs, %zu B smem, %d blocks/SM, carve-out %d %%, BVH depth %d\n", t.name, fa.numRegs,
                 fa.sharedSizeBytes + t.smem, blocksPerSM, pct, scene->bvhDepth);
-    t.grid = g_numSMs * std::max(1, std::min(blocksPerSM, 8));
+    t.grid = g_numSMs * blocksPerSM;
     *out = t;
     return PB2_OK;
 }
@@ -1035,7 +1029,7 @@ static WfPool poolOf(const pb2_scene *scene, int capacity, int pipe = 0, int nPi
 static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *film, cudaStream_t stream, int flags,
                            bool timeTrace, unsigned long long *launches, double *traceMs) {
     const bool lazyLights = scene->lazyLightDist;   // k_wf_finish cannot defer a vertex: the rounds run to the end instead
-    // 4 M contexts (1 GiB) measured best on 1920x1080: 1 M -> 160, 2 M -> 174, 4 M -> 180 Msamples/s
+    // 4 M contexts (1 GiB) at most: enough paths in flight to keep the SMs busy at 1920x1080
     static const int maxCapacity = envInt("PB2_POOL", 1 << 22);
     long long want = std::min<long long>(maxCapacity, std::max<long long>(rp.nWorkItems, 1024));
     int capacity = (int)((want + 255) / 256 * 256);
@@ -1055,7 +1049,6 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         chain.film = film;
     }
     const bool spheres = scene->d.spheres != nullptr;
-    // (12 / 16 resident blocks for the light step - 40 / 32 registers with small spills - measured: 222.5 / 220.9 against 224.0)
     AdvanceKernel advLight = spheres ? k_wf_advance<false, true, 8> : k_wf_advance<false, false, 8>;
     AdvanceKernel advShade = scene->hasSpecular ? (spheres ? k_wf_advance<true, true, 4, true> : k_wf_advance<true, false, 4, true>)
                              : spheres ? k_wf_advance<true, true, 4>
@@ -1079,31 +1072,14 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     const unsigned finishThreshold = ((flags & PB2_FLAG_COUNT_TRAVERSAL) || lazyLights || textured) ? 0u : (unsigned)(g_numSMs * std::max(0, finishPerSM));
     const int finishBlocks = std::max(1, (int)((finishThreshold + 127) / 128));
     static const int syncEvery = std::max(1, envInt("PB2_SYNC_EVERY", 8));
-    // (A persisting-L2 access-policy window over the node array was measured and lost 3.5 %: the 126 MB
-    // L2 already holds nodes + leaf records, and carving a persisting partition only shrinks what the
-    // path contexts get.)
     // Two pipelines, each with half of the contexts and its own lists, on two streams: the kernels of one fill the SMs
-    // that the other leaves idle at the end of every launch (a persistent trace launch ends with ~0.2 ms in which the last
-    // long rays finish while most warps have exited; 136 launches per frame).  Both draw samples from the one work counter.
-    // PB2_PIPES=1: one pipeline.  Lazily lit scenes share one request list: one pipeline.
-    // How many: a traversal-bound scene (1 M soup: trace 80 % of the kernel time) is best with two - 219 / 229 / 222 / 216
-    // Msamples/s with 1 / 2 / 3 / 4 pipelines - a shading-bound one (killeroo-like: trace 22 %) with four: 195 / 221 / 249 / 261.
-    // The first two frames of a scene run with two, the second one measures the trace kernel's share of the frame; later frames use four
-    // when that share is small.  PB2_PIPES fixes the number.
+    // that the other leaves idle at the end of every launch (a persistent trace launch ends with a stretch in which the last
+    // long rays finish while most warps have exited).  Both draw samples from the one work counter.
+    // Lazily lit scenes share one request list: one pipeline.  On an H100 two are faster than four on the traversal-bound
+    // soup, the shading-bound killeroo scene and the instanced scene alike.  PB2_PIPES fixes the number (1 ... 4).
     static const int pipesEnv = envInt("PB2_PIPES", 0);
-    // (not on a scene's very first frame: that one also pays for loading the kernels it is the first to launch, which
-    // inflates the frame time the share is taken of - a box with a slow host was seen to choose four pipelines for the soup)
-    const bool calibrate = pipesEnv <= 0 && scene->pipesChosen == 0 && scene->framesRendered >= 1 && !lazyLights && capacity >= 65536 &&
-                           rp.nWorkItems >= 4 * (long long)capacity;
-    scene->framesRendered++;
-    if (calibrate) timeTrace = true;
-    const int pipesWanted = std::min((int)kMaxPipes, pipesEnv > 0 ? pipesEnv : (scene->pipesChosen > 0 ? scene->pipesChosen : 2));
+    const int pipesWanted = std::min((int)kMaxPipes, pipesEnv > 0 ? pipesEnv : 2);
     const int nPipes = (lazyLights || capacity < 65536) ? 1 : pipesWanted;
-    if (calibrate) {
-        for (int k = 0; k < 2; ++k)
-            if (!scene->frameEvents[k]) CUDA_TRY(cudaEventCreate(&scene->frameEvents[k]));
-        CUDA_TRY(cudaEventRecord(scene->frameEvents[0], stream));
-    }
     cudaStream_t streams[kMaxPipes] = {stream, stream, stream, stream};
     if (nPipes > 1) {
         if (!scene->forkEvent) CUDA_TRY(cudaEventCreateWithFlags(&scene->forkEvent, cudaEventDisableTiming));
@@ -1199,18 +1175,6 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     }
     // (with two pipelines this is the sum of launch durations of kernels that each shared the GPU with the other pipeline's
     // kernels: algorithmic bytes / this time is the per-launch figure the roofline contract asks for, a conservative one)
-    if (calibrate) {
-        CUDA_TRY(cudaEventRecord(scene->frameEvents[1], stream));
-        CUDA_TRY(cudaEventSynchronize(scene->frameEvents[1]));
-        float frameMs = 0;
-        CUDA_TRY(cudaEventElapsedTime(&frameMs, scene->frameEvents[0], scene->frameEvents[1]));
-        // mean over the two pipelines of (summed duration of its trace launches) / frame: 0.41 on the 1 M soup, 0.42 on the
-        // instanced scene (two pipelines are best), 0.25 on the killeroo-like scene (four are)
-        const double share = frameMs > 0 ? *traceMs / nPipes / frameMs : 1;
-        scene->pipesChosen = share < 0.33 ? 4 : 2;
-        static const int verbose = envInt("PB2_VERBOSE", 0);
-        if (verbose) fprintf(stderr, "pb2: trace share of the calibration frame %.2f -> %d wavefront pipelines\n", share, scene->pipesChosen);
-    }
     return PB2_OK;
 }
 
@@ -1268,9 +1232,9 @@ int pb2_init_devices(int n, const int *device_ids) {
         CUDA_TRY(cudaSetDevice(id));
         cudaDeviceProp prop;
         CUDA_TRY(cudaGetDeviceProperties(&prop, id));
-        if (prop.major < 10) {
+        if (prop.major != 9 || prop.minor != 0) {   // sm_90a code loads on compute capability 9.0 only
             freeDeviceTables();
-            return setError(PB2_ERR_NO_DEVICE, std::string("device \"") + prop.name + "\" is not sm_100-class; this library is built for sm_100a only");
+            return setError(PB2_ERR_NO_DEVICE, std::string("device \"") + prop.name + "\" is not sm_90 (Hopper); this library is built for sm_90a only");
         }
         g_devs.emplace_back();
         DeviceState &d = g_devs.back();
@@ -1425,8 +1389,6 @@ int pb2_scene_destroy(pb2_scene *s) {
         if (s->joinEvents[p]) cudaEventDestroy(s->joinEvents[p]);
     }
     if (s->forkEvent) cudaEventDestroy(s->forkEvent);
-    for (int k = 0; k < 2; ++k)
-        if (s->frameEvents[k]) cudaEventDestroy(s->frameEvents[k]);
     delete s;
     if (g_initialised) cudaSetDevice(g_devs[0].id);
     return PB2_OK;
@@ -3216,7 +3178,7 @@ static int hlbvhOnDevice(const float *prim_bounds, int64_t n, int32_t max_prims_
         step(cudaMemset(dStart, 0xff, 4096 * sizeof(int)));
         step(cudaEventRecord(e0));
         const int threads = 256, blocks = (N + threads - 1) / threads;
-        k_hlbvh_centroid_bounds<<<std::min(blocks, 148 * 8), threads>>>(dBounds, N, dBox);
+        k_hlbvh_centroid_bounds<<<std::min(blocks, g_numSMs * 8), threads>>>(dBounds, N, dBox);
         k_hlbvh_morton<<<blocks, threads>>>(dBounds, N, dBox, dCodes, dIndex);
         // the reference's LSD radix sort over all 30 bits is a stable sort by the code; so is this one
         step(cub::DeviceRadixSort::SortPairs(dTemp, tempBytes, dCodes, dCodesSorted, dIndex, dSorted, N, 0, 30));
@@ -3235,7 +3197,7 @@ static int hlbvhOnDevice(const float *prim_bounds, int64_t n, int32_t max_prims_
         if (nodes && e == cudaSuccess) {
             // the SAH tree over the treelet roots and the depth-first layout, without leaving the device
             k_hlbvh_upper<<<1, 32>>>(dPool, dRoots, dTreeletNodes, nT, up, dLinear);
-            k_hlbvh_flatten<<<std::min(nT, 148 * 8), 128>>>(dPool, dTreelets, dTreeletNodes, up.treeletBase, nT, dLinear);
+            k_hlbvh_flatten<<<std::min(nT, g_numSMs * 8), 128>>>(dPool, dTreelets, dTreeletNodes, up.treeletBase, nT, dLinear);
             step(cudaGetLastError());
         }
         step(cudaEventRecord(e1));

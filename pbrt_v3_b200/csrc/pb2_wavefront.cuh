@@ -133,10 +133,8 @@ __device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfP
     return started;
 }
 
-// Contexts on the free list take their next sample.  (Letting a context whose path has ended take its next sample right
-// inside k_wf_advance - no free list, no separate launch - was measured: 225 -> 205 Msamples/s at 16 spp on the 1 M soup,
-// 187 -> 159 on the killeroo-like scene: the few lanes of a warp that end a path run this code alone inside the
-// register-heavy, low-occupancy shade kernel.)
+// Contexts on the free list take their next sample.  (Not inside k_wf_advance: there the few lanes of a warp that end a
+// path would run this code alone inside the register-heavy, low-occupancy shade kernel.)
 // GENERAL = true: the instantiation that can also draw from the SobolSampler (frames that use it).
 template <bool GENERAL>
 __global__ void __launch_bounds__(256) k_wf_gen(DRenderParams rp, WfPool pool, int freeQ, int traceQ) {
@@ -222,9 +220,9 @@ __global__ void __launch_bounds__(128) k_wf_trace_plain(DScene sc, WfPool pool, 
 //               left), then store their results, append their context to the shade / light list,
 //               and take the next rays of the trace list (one warp-aggregated atomic)
 // Node-visit and primitive-test counts per ray are the reference's; only the interleaving across
-// lanes differs.  Details that came out of ncu (profiles/):
-//   * the traversal stack lives in shared memory, [depth][thread] (conflict-free): a local-memory
-//     stack missed L1 40 % of the time; entries beyond SDEPTH spill to a small local array (DEEP),
+// lanes differs.  Details:
+//   * the traversal stack lives in shared memory, [depth][thread] (conflict-free), not in local
+//     memory, where it competes with node fetches for L1; entries beyond SDEPTH spill to a small local array (DEEP),
 //     or the host picks this kernel only when the BVH depth fits (DEEP = false);
 //   * the closest hit so far is written straight into the context (it changes ~1.5 times per ray);
 //     only tMax stays in a register -> 59 registers, 8 blocks of 128 threads per SM;
@@ -296,8 +294,6 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(DScene sc, WfPool pool, 
                     int slot = interior ? sp : (sp > 0 ? sp - 1 : 0);
                     int top = stackGet(slot);
                     if (interior) stackPut(slot, far);
-                    // (prefetching the far child here - prefetch.global.L1 / .L2, CCTL.PF1/PF2 - was
-                    // measured: -3.5 % on the bench scene, the extra L1 traffic costs more than it hides)
                     if (interior) {
                         cur = near;
                         ++sp;
@@ -487,7 +483,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(DScene sc, WfPool pool, 
 // device/pb2_wide4.cuh) - two levels of the reference's tree per fetch: a visit tests the four
 // grandchildren's boxes, continues with the first entered one in the reference's visiting order and
 // defers the others (up to three stack entries, the next one to visit on top).
-// LEAFTMA (experiment, PB2_FLAG_LEAF_TMA; measured and NOT adopted, DESIGN.md section 3): the leaf records of the lanes that
+// LEAFTMA (experiment, PB2_FLAG_LEAF_TMA; not the default, DESIGN.md section 3): the leaf records of the lanes that
 // take a leaf step are staged into shared memory by the TMA unit - one cp.async.bulk (UBLKCP) of up to four 48-byte records
 // per lane, completion counted by one mbarrier per warp - and the triangle tests read them from there.
 template <int WIDTH, int LEAF_T, int FETCH_T, int NSUB, int SDEPTH, int MINB, bool SPHERES = false, bool INST = false, bool LD256 = false,
@@ -1104,12 +1100,6 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool p
 }
 
 // ---------------------------------------------------------------------------------------------
-// (Measured and dropped, round 1: a variant of k_wf_trace with TWO rays per lane - the active ray in
-// registers, a parked one in shared memory, swapped in whenever the active ray had to wait for a
-// leaf / fetch step.  It raised the node step from 17.5 to ~20 active lanes but paid 9 % of its
-// instructions for the swaps at 5 active lanes and squeezed L1 with the second stack: -9 % overall.)
-// ---------------------------------------------------------------------------------------------
-// ---------------------------------------------------------------------------------------------
 // laneAdvance for every context of one list.  SHADE = true: the shade list (path rays: the whole
 // vertex is evaluated); SHADE = false: the light list (shadow / MIS rays: a few adds and the next
 // ray).  Two instantiations so that the light kernel is small and the warps of each stay converged.
@@ -1167,8 +1157,8 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(DScene sc, DRenderPara
 
 // ---------------------------------------------------------------------------------------------
 // End of a frame.  Once the work counter has run out the pool is no longer refilled and the number of paths in
-// flight decays round by round: ~25 more rounds, each a handful of launches over a few thousand rays that cannot
-// fill the machine (measured round 1: a fixed ~7.8 ms per frame whatever the GPU count - 10 % of a frame at 8 GPUs).
+// flight decays round by round: many more rounds, each a handful of launches over a few thousand rays that cannot
+// fill the machine - a fixed cost per frame whatever the GPU count, so a growing share of the frame on several GPUs.
 // k_wf_finish runs after the shade step of every round and does nothing until (a) no work item is left and (b) at
 // most `threshold` contexts are still in flight; then every thread takes ONE of them and walks it to the end of its
 // path with the per-lane state machine (traceLane + laneAdvance, the code of k_li_samples / pb2_li_samples), deposits

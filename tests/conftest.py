@@ -11,7 +11,7 @@ SCENES = os.path.join(ROOT, "tests", "scenes")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -27,16 +27,6 @@ def port():
     o = pyoracle.port()
     if o is None:
         pytest.fail("oracle/lib/libpb2_oracle.so is missing: run __graft_entry__.build()")
-    return o
-
-
-@pytest.fixture(scope="session")
-def reference():
-    """The compiled reference (oracle/_ref). Only exists where /root/reference was available at build time."""
-    from oracle import pyoracle
-    o = pyoracle.reference()
-    if o is None:
-        pytest.skip("oracle/_ref not built (no /root/reference on this machine)")
     return o
 
 

@@ -1,4 +1,6 @@
 """Seeded inputs shared by tests/make_golden.py (which records the reference's outputs for them) and the tests."""
+import os
+
 import numpy as np
 
 SOUP = dict(n_tris=2000, seed=77, jitter=0.05, xres=32, yres=18, spp=4, maxdepth=5)
@@ -210,6 +212,7 @@ DIFFERENTIAL_SCENES = ("textured", "textured_lens", "bumpmap", "instances")
 
 
 BSDF_SCENES = ("materials", "specular", "substrate", "metal", "uber", "roughglass")
+BSDF_FRAMES = 1000   # shading frames per material record (the fixture stays under 1 MB)
 
 
 def bsdf_frames(n, seed):
@@ -227,3 +230,39 @@ def bsdf_frames(n, seed):
     dpdu[::4] += 0.2 * ns[::4]
     wo, wi = unit(rs.normal(size=(n, 3))), unit(rs.normal(size=(n, 3)))
     return np.ascontiguousarray(np.concatenate([nrm, ns, dpdu, wo, wi, rs.uniform(0, 1, (n, 2))], 1), np.float32)
+
+
+def lights_text(scene_dir, strategy):
+    """tests/scenes/lights.pbrt under another light-sampling strategy ("spatial", "uniform")."""
+    text = open(os.path.join(scene_dir, "lights.pbrt")).read()
+    return text.replace('"string lightsamplestrategy" "power"', '"string lightsamplestrategy" "%s"' % strategy)
+
+
+def awkward_textures(pb):
+    """Random images of awkward sizes (1 x N, N x 1, primes, already a power of two) as pb2_texture records; the texel
+    arrays are kept alive on the records."""
+    import ctypes as C
+    rs = np.random.RandomState(9)
+    out = []
+    for (w, h, ch, wrap) in [(1, 1, 1, 0), (1, 7, 3, 0), (5, 1, 1, 2), (13, 31, 3, 1), (16, 4, 1, 0), (33, 64, 3, 2), (100, 3, 1, 1)]:
+        texels = rs.uniform(0, 2, (h, w, ch)).astype(np.float32)
+        t = pb.Texture(channels=ch, width=w, height=h, wrap=wrap, do_trilinear=0, max_anisotropy=8.0, su=1, sv=1, du=0, dv=0,
+                       texels=texels.ctypes.data_as(C.POINTER(C.c_float)))
+        t._texels = texels
+        out.append(t)
+    return out
+
+
+# the reference's scenes/killeroo-simple.pbrt and the file it includes, stored in tests/golden/killeroo_simple.npz
+KILLEROO_FILES = {"scene": "killeroo-simple.pbrt", "geometry": os.path.join("geometry", "killeroo.pbrt")}
+
+
+def killeroo_scene(directory, golden_dir):
+    """Writes the stored killeroo-simple scene into `directory` (its Include is relative) and returns the scene file's path."""
+    g = np.load(os.path.join(golden_dir, "killeroo_simple.npz"))
+    for key, rel in KILLEROO_FILES.items():
+        path = os.path.join(directory, rel)
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, "wb") as f:
+            f.write(g[key].tobytes())
+    return os.path.join(directory, KILLEROO_FILES["scene"])

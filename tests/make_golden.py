@@ -1,10 +1,11 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (oracle/_ref, built from /root/reference by
-oracle/Makefile.ref) on the seeded inputs of tests/golden_cases.py.  Run in the build container:
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (oracle/_ref, built by oracle/Makefile.ref) on the
+seeded inputs of tests/golden_cases.py, and stores a few data files of the reference (a scene, image test files).
+Run where the reference's source tree is, after __graft_entry__.build():
 
-    python tests/make_golden.py
+    PBRT_V3_DIR=<the reference's source tree> python tests/make_golden.py
 
-The fixtures travel with the repo; the tests compare the oracle port (everywhere) and the CUDA path (on the GPU box)
-against them, so that parity is pinned to the reference even where /root/reference does not exist.
+The fixtures travel with the repo; the tests compare the oracle port (everywhere) and the CUDA path (on a GPU)
+against them, so that parity is pinned to the reference where it does not exist.
 """
 import os
 import sys
@@ -134,7 +135,7 @@ def record_bsdfs(ref):
         hs = pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", scene + ".pbrt"))
         d = hs.desc.contents
         for m in range(d.n_materials):
-            out["%s_%d" % (scene, m)] = ref.bsdf_eval(d.materials[m], gc.bsdf_frames(1500, 17 + m))
+            out["%s_%d" % (scene, m)] = ref.bsdf_eval(d.materials[m], gc.bsdf_frames(gc.BSDF_FRAMES, 17 + m))
     np.savez_compressed(os.path.join(OUT, "bsdf.npz"), **out)
     print("bsdf:", len(out), "materials")
 
@@ -149,10 +150,82 @@ def record_env_distribution(ref):
     print("env distribution", nu, nv)
 
 
+def record_texture_pyramids(ref):
+    """MIPMap::pyramid of the reference for random images of awkward sizes (tests/golden_cases.py AWKWARD_TEXTURES)."""
+    out = {}
+    for i, t in enumerate(gc.awkward_textures(pb)):
+        levels = ref.texture_pyramid(t)
+        out["levels_%d" % i] = np.array([[lv.shape[1], lv.shape[0]] for lv in levels], np.int32)
+        out["pyramid_%d" % i] = np.concatenate([lv.ravel() for lv in levels])
+    np.savez_compressed(os.path.join(OUT, "texture_pyramids.npz"), **out)
+    print("texture pyramids:", len(out) // 2, "images")
+
+
+def record_sobol_tables(ref):
+    """The reference's SobolMatrices32 and its VdCSobolMatrices / VdCSobolMatricesInv for every resolution 2^1 ... 2^25."""
+    _, mats = ref.sobol_tables(1)
+    tabs = np.stack([ref.sobol_tables(m)[0] for m in range(1, 26)])
+    np.savez_compressed(os.path.join(OUT, "sobol_tables.npz"), matrices=mats, vdc=tabs)
+    print("sobol tables", mats.shape, tabs.shape)
+
+
+def record_killeroo_scene(ref_dir):
+    """The reference's scenes/killeroo-simple.pbrt and the geometry it includes, stored as bytes (scene data, no source)."""
+    scenes = os.path.join(ref_dir, "scenes")
+    np.savez_compressed(os.path.join(OUT, "killeroo_simple.npz"),
+                        **{k: np.frombuffer(open(os.path.join(scenes, rel), "rb").read(), np.uint8) for k, rel in gc.KILLEROO_FILES.items()})
+    print("killeroo-simple scene stored")
+
+
+def crop_exr(data, n_lines):
+    """A single-part scan-line OpenEXR file cut to its first n_lines: the header with a shorter data window, the line blocks
+    that cover those lines (OpenEXR's own bytes) and a new offset table."""
+    import struct
+    lines_per_block = {0: 1, 1: 1, 2: 1, 3: 16, 4: 32, 6: 32}
+    pos, comp, window = 8, None, None
+    while data[pos] != 0:
+        name_end = data.index(b"\0", pos)
+        type_end = data.index(b"\0", name_end + 1)
+        name, size = data[pos:name_end], struct.unpack_from("<i", data, type_end + 1)[0]
+        pos = type_end + 5
+        if name == b"compression":
+            comp = data[pos]
+        elif name == b"dataWindow":
+            window = pos
+        pos += size
+    header = bytearray(data[:pos + 1])
+    x0, y0, x1, y1 = struct.unpack_from("<4i", data, window)
+    struct.pack_into("<4i", header, window, x0, y0, x1, y0 + n_lines - 1)
+    lpb = lines_per_block[comp]
+    offsets = struct.unpack_from("<%dQ" % ((y1 - y0 + lpb) // lpb), data, pos + 1)
+    chunks = [data[o:o + 8 + struct.unpack_from("<i", data, o + 4)[0]] for o in offsets[:(n_lines + lpb - 1) // lpb]]
+    table, offset = b"", len(header) + 8 * len(chunks)
+    for c in chunks:
+        table += struct.pack("<Q", offset)
+        offset += len(c)
+    return bytes(header) + table + b"".join(chunks)
+
+
+def record_openexr_images(ref_dir):
+    """OpenEXR's own test images bundled with the reference (src/ext/openexr/OpenEXR/IlmImfTest): one picture uncompressed
+    and under the RLE / ZIPS / ZIP / PIZ / B44 codecs, cut to its first 32 lines (the whole files are over 1 MB), and a PIZ
+    file stored in both line orders, whole (the decreasing one keeps its blocks bottom-up)."""
+    src = os.path.join(ref_dir, "src", "ext", "openexr", "OpenEXR", "IlmImfTest")
+    os.makedirs(os.path.join(OUT, "openexr"), exist_ok=True)
+    for name in ("comp_none", "comp_rle", "comp_zips", "comp_zip", "comp_piz", "comp_b44", "lineOrder_increasing", "lineOrder_decreasing"):
+        data = open(os.path.join(src, name + ".exr"), "rb").read()
+        with open(os.path.join(OUT, "openexr", name + ".exr"), "wb") as f:
+            f.write(crop_exr(data, 32) if name.startswith("comp_") else data)
+    print("openexr test images stored")
+
+
 def main():
+    ref_dir = os.environ.get("PBRT_V3_DIR")
+    if not ref_dir or not os.path.isdir(os.path.join(ref_dir, "src")):
+        raise SystemExit("set PBRT_V3_DIR to the reference's source tree (the directory that holds src/ and scenes/)")
     ref = pyoracle.reference()
     if ref is None:
-        raise SystemExit("oracle/_ref is not built: run `make -C oracle -f Makefile.ref` where /root/reference exists")
+        raise SystemExit("oracle/_ref is not built: run `make -C oracle -f Makefile.ref REF=$PBRT_V3_DIR`")
     os.makedirs(OUT, exist_ok=True)
     record_scene(ref, gc.soup_scene(pb), "soup")
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "killeroo_like.pbrt")), "killeroo_like")
@@ -164,6 +237,8 @@ def main():
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "uber.pbrt")), "uber")
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "roughglass.pbrt")), "roughglass")
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "lights.pbrt")), "lights")
+    for strategy in ("spatial", "uniform"):
+        record_scene(ref, pb.HostScene.from_string(gc.lights_text(os.path.join(ROOT, "tests", "scenes"), strategy)), "lights_" + strategy)
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "params.pbrt")), "params")
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "envlight.pbrt")), "envlight")
     record_scene(ref, pb.HostScene.from_file(os.path.join(ROOT, "tests", "scenes", "textured.pbrt")), "textured")
@@ -178,6 +253,10 @@ def main():
     record_bsdfs(ref)
     record_env_distribution(ref)
     record_textures(ref)
+    record_texture_pyramids(ref)
+    record_sobol_tables(ref)
+    record_killeroo_scene(ref_dir)
+    record_openexr_images(ref_dir)
     record_filters(ref)
     record_hlbvh(ref)
     # the metal material's default eta / k: copper's measured spectra through Spectrum::FromSampled (metal.cpp:121-126)

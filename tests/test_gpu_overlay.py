@@ -1,5 +1,5 @@
 """INTEGRATION.md's binding, compiled against the reference's own classes (oracle/overlay_b200path.cpp ->
-oracle/_ref/libb200_overlay.so, built where /root/reference exists): a `B200PathIntegrator : pbrt::Integrator` flattens a
+oracle/_ref/libb200_overlay.so, built where the reference's sources are): a `B200PathIntegrator : pbrt::Integrator` flattens a
 REFERENCE Scene (BVHAccel, Triangle, Sphere, MatteMaterial / PlasticMaterial, DiffuseAreaLight, Film, PerspectiveCamera,
 HaltonSampler objects of the reference) into a pb2_scene_desc, renders through libpb2.so and merges the film through the
 reference's Film::MergeFilmTile / WriteImage.  Its image must match the reference's PathIntegrator on the same Scene."""
@@ -18,7 +18,7 @@ OVERLAY = os.path.join(ROOT, "oracle", "_ref", "libb200_overlay.so")
 @pytest.mark.parametrize("name", ["soup", "soup_sobol", "killeroo_like", "materials_matte_plastic"])
 def test_reference_scene_through_the_b200_integrator(pb, name):
     if not os.path.exists(OVERLAY):
-        pytest.skip("oracle/_ref/libb200_overlay.so not built (no /root/reference at build time)")
+        pytest.skip("oracle/_ref/libb200_overlay.so not built (no reference sources at build time)")
     from pbrt_v3_b200 import Camera, FilmDesc, PathParams, SceneDesc, Stats
     pb.init()
     L = C.CDLL(OVERLAY)

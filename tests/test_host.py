@@ -813,8 +813,8 @@ def test_openexr_reader(pb, tmp_path):
     """ReadImage for OpenEXR scan-line files (imageio.cpp:125-151 reads them through OpenEXR's RgbaInputFile): half channels
     stored B, G, R; ZIP blocks of 16 lines (the last one short) with the byte-delta predictor and the even / odd byte split,
     blocks stored raw when they do not shrink, uncompressed files, and the PIZ codec - the committed files of tests/scenes/make_textures.py,
-    the container this library writes itself, and (where the reference's bundled OpenEXR sources are present) OpenEXR's own
-    test images, which hold one picture under every codec."""
+    the container this library writes itself, and OpenEXR's own test images (tests/golden/openexr): one picture under every
+    codec (its first 32 lines) and a PIZ file stored in both line orders."""
     tex = os.path.join(SCENES, "textures")
     want = np.load(os.path.join(tex, "decoded_8bit.npz"))["exr"]
     for kind in ("zip", "zips", "none"):
@@ -830,16 +830,15 @@ def test_openexr_reader(pb, tmp_path):
                                   'Material "matte" "texture Kd" "t"\nShape "sphere"\nWorldEnd\n' % tex)
     t = hs.desc.contents.textures[0]
     assert np.array_equal(np.ctypeslib.as_array(t.texels, shape=(18, 24, 3)), want[::-1])
-    ilm = "/root/reference/src/ext/openexr/OpenEXR/IlmImfTest"
-    if os.path.exists(os.path.join(ilm, "comp_none.exr")):
-        base = pb.read_image(os.path.join(ilm, "comp_none.exr"))
-        assert base.shape == (675, 587, 3) and np.isfinite(base).all()
-        for codec in ("rle", "zips", "zip", "piz"):      # piz: value table + wavelet + Huffman with run lengths
-            assert np.array_equal(pb.read_image(os.path.join(ilm, "comp_%s.exr" % codec)).view(np.uint32), base.view(np.uint32)), codec
-        up, down = (pb.read_image(os.path.join(ilm, "lineOrder_%s.exr" % o)) for o in ("increasing", "decreasing"))   # PIZ, 119 lines
-        assert up.shape == (119, 237, 3) and np.array_equal(up.view(np.uint32), down.view(np.uint32))
-        # the lossy codecs are reported, not misread
-        before = pb.lib().pb2h_error_count()
-        with pytest.raises(RuntimeError):
-            pb.read_image(os.path.join(ilm, "comp_b44.exr"))
-        assert pb.lib().pb2h_error_count() > before
+    ilm = os.path.join(GOLDEN, "openexr")
+    base = pb.read_image(os.path.join(ilm, "comp_none.exr"))
+    assert base.shape == (32, 587, 3) and np.isfinite(base).all()
+    for codec in ("rle", "zips", "zip", "piz"):      # piz: value table + wavelet + Huffman with run lengths
+        assert np.array_equal(pb.read_image(os.path.join(ilm, "comp_%s.exr" % codec)).view(np.uint32), base.view(np.uint32)), codec
+    up, down = (pb.read_image(os.path.join(ilm, "lineOrder_%s.exr" % o)) for o in ("increasing", "decreasing"))   # PIZ, 119 lines
+    assert up.shape == (119, 237, 3) and np.array_equal(up.view(np.uint32), down.view(np.uint32))
+    # the lossy codecs are reported, not misread
+    before = pb.lib().pb2h_error_count()
+    with pytest.raises(RuntimeError):
+        pb.read_image(os.path.join(ilm, "comp_b44.exr"))
+    assert pb.lib().pb2h_error_count() > before

@@ -1,6 +1,7 @@
 """The CPU oracle (oracle/pb2_oracle.cpp) against (a) golden vectors recorded from the unmodified reference
 (tests/make_golden.py), (b) the reference's own known-answer tests for this path (src/tests/shapes.cpp,
-src/tests/sampling.cpp), and (c) where it exists, the compiled reference itself (oracle/_ref), live.
+src/tests/sampling.cpp), and (c) the compiled reference itself (oracle/_ref) where it was built - elsewhere the `_live`
+tests compare with the same reference's recorded outputs.
 Everything here runs on the CPU; bit-exact unless said otherwise.
 """
 import os
@@ -63,10 +64,18 @@ def test_port_matches_reference_golden(pb, port, name):
     assert same_bvh(nodes, g["bvh_nodes"]) and np.array_equal(prims, g["bvh_prims"]), "BVHAccel linear nodes + primitive order"
 
 
+def reference_outputs(pb, hs, golden_name):
+    """What the reference computes for `hs`: the compiled reference (oracle/_ref) where it was built, else its outputs
+    recorded by tests/make_golden.py (tests/golden/<golden_name>.npz, same keys as recompute())."""
+    from oracle import pyoracle
+    ref = pyoracle.reference()
+    return recompute(pb, ref, hs) if ref is not None else np.load(os.path.join(GOLDEN, golden_name + ".npz"))
+
+
 @pytest.mark.parametrize("name", SCENE_CASES)
-def test_port_matches_compiled_reference_live(pb, port, reference, name):
+def test_port_matches_compiled_reference_live(pb, port, name):
     hs = load_scene(pb, name)
-    a, b = recompute(pb, reference, hs), recompute(pb, port, hs)
+    a, b = reference_outputs(pb, hs, name), recompute(pb, port, hs)
     for k in ("hits", "occluded", "halton", "light_distribution", "li", "pfilm", "image", "rays"):
         assert a[k].tobytes() == b[k].tobytes(), k
 
@@ -82,18 +91,20 @@ def test_port_filters_match_reference_golden(pb, port, case):
 
 
 @pytest.mark.parametrize("strategy", ["spatial", "uniform"])
-def test_port_delta_lights_other_strategies_live(pb, port, reference, strategy):
-    text = open(os.path.join(SCENES, "lights.pbrt")).read().replace('"string lightsamplestrategy" "power"', '"string lightsamplestrategy" "%s"' % strategy)
-    hs = pb.HostScene.from_string(text)
-    a, b = recompute(pb, reference, hs), recompute(pb, port, hs)
+def test_port_delta_lights_other_strategies_live(pb, port, strategy):
+    hs = pb.HostScene.from_string(gc.lights_text(SCENES, strategy))
+    a, b = reference_outputs(pb, hs, "lights_" + strategy), recompute(pb, port, hs)
     for k in ("light_distribution", "li", "image", "rays"):
         assert a[k].tobytes() == b[k].tobytes(), k
 
 
-def test_port_filters_match_compiled_reference_live(pb, port, reference):
+def test_port_filters_match_compiled_reference_live(pb, port):
+    from oracle import pyoracle
+    ref = pyoracle.reference()
+    g = np.load(os.path.join(GOLDEN, "filters.npz"))
     for case in sorted(gc.FILTER_CASES):
         hs = pb.HostScene.from_string(gc.filter_scene_text(SCENES, case))
-        a, _, _ = reference.scene(hs).render(n_threads=1)
+        a = ref.scene(hs).render(n_threads=1)[0] if ref is not None else g["image_" + case]
         b, _, _ = port.scene(hs).render(n_threads=1)
         assert a.tobytes() == b.tobytes(), case
 
@@ -286,21 +297,17 @@ def test_empty_and_degenerate_inputs(pb, port):
     assert h["prim"][0] >= 0 and h["prim"][1] == -1 and h["prim"][2] == -1
 
 
-def test_killeroo_simple_fingerprint_of_the_surveyed_reference(pb, reference, tmp_path):
+def test_killeroo_simple_fingerprint_of_the_surveyed_reference(pb, checker, tmp_path):
     """SURVEY.md section 9: `pbrt --outfile k8.pfm scenes/killeroo-simple.pbrt` of the reference binary gives md5
-    5424ce0f17db0c040e0f988ebcfe4b4d with 16 870 506 regular + 6 157 124 shadow ray tests.  The same file parsed by
-    THIS repo's host front end (parser, loop subdivision, transforms, SAH BVH builder), rendered by oracle/_ref (the
-    reference's own sources behind ref_harness.cpp) and written by our PFM writer must give those bytes: one test pins
-    the harness, the parser, the subdivision and the builder to the surveyed binary."""
+    5424ce0f17db0c040e0f988ebcfe4b4d with 16 870 506 regular + 6 157 124 shadow ray tests.  The same file (stored in
+    tests/golden/killeroo_simple.npz) parsed by THIS repo's host front end (parser, loop subdivision, transforms, SAH BVH
+    builder), rendered by the CPU checker and written by our PFM writer must give those bytes: one test pins the checker,
+    the parser, the subdivision and the builder to the surveyed binary."""
     import hashlib
-    from conftest import ROOT
-    scene = os.path.join(ROOT, "baseline", "_scenes", "killeroo-simple.pbrt")
-    if not os.path.exists(scene):
-        pytest.skip("baseline/_scenes/killeroo-simple.pbrt not staged (no /root/reference at build time)")
-    hs = pb.HostScene.from_file(scene)
+    hs = pb.HostScene.from_file(gc.killeroo_scene(str(tmp_path), GOLDEN))
     d = hs.desc.contents
     assert d.n_prims == 66533 and d.n_nodes == 59188 + 59189
-    img, _, st = reference.scene(hs).render(n_threads=0)
+    img, _, st = checker.scene(hs).render(n_threads=0)
     assert img.shape == (700, 700, 3)
     assert (int(st.camera_rays), int(st.regular_rays), int(st.shadow_rays)) == (3920000, 16870506, 6157124)
     out = str(tmp_path / "k8.pfm")
@@ -327,18 +334,21 @@ def test_library_texture_pyramids_are_the_reference_mipmaps(pb):
     assert resampled >= 4
 
 
-def test_library_texture_pyramids_match_reference_live(pb, reference):
-    """... and against the reference live, on random images of awkward sizes (1 x N, N x 1, primes, already a power of two)."""
-    import ctypes as C
-    rs = np.random.RandomState(9)
-    for (w, h, ch, wrap) in [(1, 1, 1, 0), (1, 7, 3, 0), (5, 1, 1, 2), (13, 31, 3, 1), (16, 4, 1, 0), (33, 64, 3, 2), (100, 3, 1, 1)]:
-        texels = rs.uniform(0, 2, (h, w, ch)).astype(np.float32)
-        t = pb.Texture(channels=ch, width=w, height=h, wrap=wrap, do_trilinear=0, max_anisotropy=8.0, su=1, sv=1, du=0, dv=0,
-                       texels=texels.ctypes.data_as(C.POINTER(C.c_float)))
-        a, b = pb.texture_pyramid(t), reference.texture_pyramid(t)
-        assert len(a) == len(b)
-        for la, lb in zip(a, b):
-            assert la.shape == lb.shape and np.array_equal(gc.bits(la), gc.bits(lb)), (w, h, ch, wrap)
+def test_library_texture_pyramids_match_reference_live(pb):
+    """... and on random images of awkward sizes (1 x N, N x 1, primes, already a power of two) against MIPMap::pyramid of
+    the compiled reference where it was built, else as recorded from it (tests/golden/texture_pyramids.npz)."""
+    from oracle import pyoracle
+    ref = pyoracle.reference()
+    g = np.load(os.path.join(GOLDEN, "texture_pyramids.npz"))
+    for i, t in enumerate(gc.awkward_textures(pb)):
+        levels = pb.texture_pyramid(t)
+        if ref is not None:
+            want = ref.texture_pyramid(t)
+            want_levels, want_texels = np.array([[lv.shape[1], lv.shape[0]] for lv in want], np.int32), np.concatenate([lv.ravel() for lv in want])
+        else:
+            want_levels, want_texels = g["levels_%d" % i], g["pyramid_%d" % i]
+        assert np.array_equal(np.array([[lv.shape[1], lv.shape[0]] for lv in levels], np.int32), want_levels), i
+        assert np.array_equal(gc.bits(np.concatenate([lv.ravel() for lv in levels])), gc.bits(want_texels)), i
 
 
 def test_sobol_sampler_matches_reference_golden(pb):
@@ -355,14 +365,15 @@ def test_sobol_sampler_matches_reference_golden(pb):
     assert (hdim < 2).sum() > 10 and (got[hdim < 2] < 1).all()
 
 
-def test_sobol_tables_are_the_reference_tables(pb, reference):
+def test_sobol_tables_are_the_reference_tables(pb):
     """The generator matrices (from scipy's copy of the Joe-Kuo direction numbers) equal the reference's SobolMatrices32, and
     the two SobolIntervalToIndex tables the library derives from dimensions 0 and 1 by inverting a matrix over GF(2) equal
-    VdCSobolMatrices / VdCSobolMatricesInv for every resolution from 2 to 2^25 pixels."""
+    VdCSobolMatrices / VdCSobolMatricesInv for every resolution from 2 to 2^25 pixels (both recorded from the compiled
+    reference: tests/golden/sobol_tables.npz)."""
     import ctypes as C
+    g = np.load(os.path.join(GOLDEN, "sobol_tables.npz"))
     mats = np.fromfile(os.path.join(os.path.dirname(pb.__file__), "lib", "sobol_matrices32.bin"), "<u4").reshape(1024, 52)
-    _, ref_mats = reference.sobol_tables(1)
-    assert np.array_equal(mats, ref_mats)
+    assert np.array_equal(mats, g["matrices"])
     film = pb.FilmDesc()
     film.filter_radius[0] = film.filter_radius[1] = 0.5
     pp = pb.PathParams(samples_per_pixel=1, sampler=pb.PB2_SAMPLER_SOBOL)
@@ -371,8 +382,7 @@ def test_sobol_tables_are_the_reference_tables(pb, reference):
         film.full_resolution[0], film.full_resolution[1] = res, 1
         film.cropped_pixel_bounds[0], film.cropped_pixel_bounds[1], film.cropped_pixel_bounds[2], film.cropped_pixel_bounds[3] = 0, 0, res, 1
         _, tab = pb.sobol_samples_host(C.byref(film), C.byref(pp), np.zeros((1, 2), np.int32), np.zeros(1, np.int64), np.zeros(1, np.int32), tables=True)
-        want, _ = reference.sobol_tables(m)
-        assert np.array_equal(tab, want), m
+        assert np.array_equal(tab, g["vdc"][m - 1]), m
 
 
 def test_environment_map_distribution_is_the_reference_distribution(pb):
@@ -437,7 +447,7 @@ def test_ray_differentials_match_the_reference(pb, scene):
 def test_shade_kernel_bsdf_functions_match_the_reference_bsdf(pb, scene):
     """The functions the shade kernel compiles - makeBsdf (matte with and without sigma, plastic, substrate, metal, uber with
     opacity / Kr / Kt, mirror, smooth and rough glass), bsdfF, bsdfPdf, bsdfSampleF - evaluated on the host for every material
-    record of a scene at 1500 random shading frames: f and Pdf over the non-specular lobes, the non-specular Sample_f of
+    record of a scene at 1000 random shading frames: f and Pdf over the non-specular lobes, the non-specular Sample_f of
     EstimateDirect and the all-lobes Sample_f of the path's continuation (direction, value, pdf, sampled flags) are BIT FOR BIT
     what the reference's Material::ComputeScatteringFunctions + BSDF return (tests/golden/bsdf.npz)."""
     g = np.load(os.path.join(GOLDEN, "bsdf.npz"))
@@ -445,7 +455,7 @@ def test_shade_kernel_bsdf_functions_match_the_reference_bsdf(pb, scene):
     d = hs.desc.contents
     types = set()
     for m in range(d.n_materials):
-        got = pb.bsdf_eval_host(d.materials[m], gc.bsdf_frames(1500, 17 + m))
+        got = pb.bsdf_eval_host(d.materials[m], gc.bsdf_frames(gc.BSDF_FRAMES, 17 + m))
         want = g["%s_%d" % (scene, m)]
         same = gc.bits(got) == gc.bits(want)
         same[:, 18] |= want[:, 17] == 0          # the sampled flags mean something only when a direction was sampled

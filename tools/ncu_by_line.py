@@ -1,6 +1,6 @@
 """Attributes the SASS-level metrics of one kernel (ncu --page source --csv) to CUDA source lines.
 
-usage:  cuobjdump -xelf all lib/libpb2.so; nvdisasm -g -c pb2_cuda.sm_100a.cubin > dis.txt
+usage:  cuobjdump -xelf all lib/libpb2.so; nvdisasm -g -c pb2_cuda.sm_90a.cubin > dis.txt
         ncu -i rep.ncu-rep --page source --csv > src.csv      (one kernel; cut the file if it holds several)
         python tools/ncu_by_line.py dis.txt src.csv <mangled-kernel-name-substring>
 The disassembly and the profile must come from the same build: instructions are matched by position."""
