@@ -413,7 +413,7 @@ struct pb2_scene {
     int wfCapacity = 0;
     std::vector<cudaEvent_t> traceEvents;
     int2 *wfSpill = nullptr;                 // k_wf_trace_pool: stack entries beyond its shared-memory depth
-    void *chainBuf = nullptr;                // device copies of {DScene, DRenderParams} for the CHAIN trace kernels
+    void *paramBuf = nullptr;                // device copies of {DScene, DRenderParams} of the render in flight (renderWavefront)
     cudaStream_t pipeStreams[4] = {nullptr, nullptr, nullptr, nullptr};   // streams of the wavefront pipelines 1.. (renderWavefront)
     cudaEvent_t forkEvent = nullptr, joinEvents[4] = {nullptr, nullptr, nullptr, nullptr};
 };
@@ -880,7 +880,7 @@ static int validateRenderArgs(const pb2_scene *scene, const pb2_camera *cam, con
 
 enum { kMaxPipes = 4 };   // wavefront pipelines (renderWavefront)
 typedef void (*TraceKernel)(DScene, WfPool, int, WfChain);
-typedef void (*AdvanceKernel)(DScene, DRenderParams, WfPool, int, int, int, float4 *, unsigned long long *);
+typedef void (*AdvanceKernel)(const DScene *, const DRenderParams *, WfPool, int, int, int, float4 *, unsigned long long *);
 
 // Which traversal kernel a scene is traced with (pb2_wavefront.cuh), and its launch shape.
 //   default                   k_wf_trace_w<2>: persistent warps over the two-child records (a record is read as
@@ -1037,15 +1037,18 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     if (rc) return rc;
     TraceLaunch trace;
     if ((rc = selectTraceKernel(scene, flags, &trace, true))) return rc;
+    // the scene and this frame's parameters as objects in device memory, read by the gen / advance / finish kernels and
+    // wfChainLight.  One buffer per scene, and so per device: every device of a group renders its own replica.
+    if (!scene->paramBuf) CUDA_TRY(cudaMalloc(&scene->paramBuf, sizeof(DScene) + sizeof(DRenderParams)));
+    const DScene *dSc = reinterpret_cast<const DScene *>(scene->paramBuf);
+    const DRenderParams *dRp = reinterpret_cast<const DRenderParams *>((char *)scene->paramBuf + sizeof(DScene));
+    CUDA_TRY(cudaMemcpyAsync((void *)dSc, &scene->d, sizeof(DScene), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync((void *)dRp, &rp, sizeof(DRenderParams), cudaMemcpyHostToDevice, stream));
     WfChain chain;
     memset(&chain, 0, sizeof(chain));
     if (trace.chain) {
-        // the scene and this frame's parameters as objects in device memory for wfChainLight
-        if (!scene->chainBuf) CUDA_TRY(cudaMalloc(&scene->chainBuf, sizeof(DScene) + sizeof(DRenderParams)));
-        CUDA_TRY(cudaMemcpyAsync(scene->chainBuf, &scene->d, sizeof(DScene), cudaMemcpyHostToDevice, stream));
-        CUDA_TRY(cudaMemcpyAsync((char *)scene->chainBuf + sizeof(DScene), &rp, sizeof(DRenderParams), cudaMemcpyHostToDevice, stream));
-        chain.sc = reinterpret_cast<const DScene *>(scene->chainBuf);
-        chain.rp = reinterpret_cast<const DRenderParams *>((char *)scene->chainBuf + sizeof(DScene));
+        chain.sc = dSc;
+        chain.rp = dRp;
         chain.film = film;
     }
     const bool spheres = scene->d.spheres != nullptr;
@@ -1063,7 +1066,7 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     const bool sobol = rp.halton.sobol != nullptr;
     const bool textured = scene->d.nTextures > 0 || sobol;
     if (textured) advShade = k_wf_advance<true, true, 3, true, true, true>;
-    typedef void (*FinishKernel)(DScene, DRenderParams, WfPool, int, unsigned, float4 *);
+    typedef void (*FinishKernel)(const DScene *, const DRenderParams *, WfPool, int, unsigned, float4 *);
     FinishKernel finish = scene->hasSpecular ? (spheres ? k_wf_finish<true, true> : k_wf_finish<false, true>)
                                              : (spheres ? k_wf_finish<true, false> : k_wf_finish<false, false>);
     // the frame's last paths are walked to their end by one thread each once this few are left (k_wf_finish)
@@ -1094,6 +1097,8 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     WfPool pools[kMaxPipes];
     for (int p = 0; p < nPipes; ++p) pools[p] = poolOf(scene, capacity / nPipes * nPipes, p, nPipes);
     const int capP = pools[0].capacity;
+    // The list kernels' grid-stride grids stay oversubscribed: grids of resident size (SMs x occupancy) for gen, light and
+    // shade were not faster on C2 (173.5 against 173.9 Msamples/s, medians of three, H100 80GB HBM3 at 700 W)
     const int blocks256 = std::min((capP + 255) / 256, g_numSMs * 16);
     const int blocks128 = std::min((capP + 127) / 128, g_numSMs * 32);
     for (int p = 0; p < nPipes; ++p) k_wf_init<<<(capP + 255) / 256, 256, 0, streams[p]>>>(pools[p]);
@@ -1107,8 +1112,8 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         for (int p = 0; p < nPipes; ++p) {
             const WfPool &pool = pools[p];
             cudaStream_t st = streams[p];
-            if (sobol) k_wf_gen<true><<<blocks256, 256, 0, st>>>(rp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
-            else k_wf_gen<false><<<blocks256, 256, 0, st>>>(rp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
+            if (sobol) k_wf_gen<true><<<blocks256, 256, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
+            else k_wf_gen<false><<<blocks256, 256, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
             if (timeTrace) {
                 if (scene->traceEvents.size() < nEvents + 2) {
                     cudaEvent_t e0, e1;
@@ -1125,16 +1130,16 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
                 CUDA_TRY(cudaEventRecord(scene->traceEvents[nEvents + 1], st));
                 nEvents += 2;
             }
-            if (!trace.chain) advLight<<<blocks128, 128, 0, st>>>(scene->d, rp, pool, WQ_LIGHT, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
+            if (!trace.chain) advLight<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_LIGHT, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
             else --nLaunch;
-            advShade<<<blocks128, 128, 0, st>>>(scene->d, rp, pool, WQ_SHADE, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
+            advShade<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_SHADE, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
             if (lazyLights) {
                 // vertices that fell into voxels without a light distribution yet were put aside: build those records, shade again
                 launchLightDistBuild(scene, st);
-                advShade<<<blocks128, 128, 0, st>>>(scene->d, rp, pool, WQ_RETRY, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
+                advShade<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_RETRY, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
                 nLaunch += 3;
             }
-            if (finishThreshold) finish<<<finishBlocks, 128, 0, st>>>(scene->d, rp, pool, WQ_TRACE0 + next, finishThreshold, film);
+            if (finishThreshold) finish<<<finishBlocks, 128, 0, st>>>(dSc, dRp, pool, WQ_TRACE0 + next, finishThreshold, film);
             k_wf_reset<<<1, 32, 0, st>>>(rp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur, WQ_TRACE0 + next, finishThreshold);
             nLaunch += finishThreshold ? 6 : 5;
         }
@@ -1383,7 +1388,7 @@ int pb2_scene_destroy(pb2_scene *s) {
     if (s->ldHostCounters) cudaFreeHost(s->ldHostCounters);
     for (cudaEvent_t e : s->traceEvents) cudaEventDestroy(e);
     if (s->wfSpill) cudaFree(s->wfSpill);
-    if (s->chainBuf) cudaFree(s->chainBuf);
+    if (s->paramBuf) cudaFree(s->paramBuf);
     for (int p = 0; p < 4; ++p) {
         if (s->pipeStreams[p]) cudaStreamDestroy(s->pipeStreams[p]);
         if (s->joinEvents[p]) cudaEventDestroy(s->joinEvents[p]);

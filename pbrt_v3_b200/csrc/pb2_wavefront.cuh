@@ -46,6 +46,20 @@ struct WfPool {
     int2 *spill;              // k_wf_trace_pool: stack entries beyond its shared-memory depth, [warp][slot][PL_SPILL]
 };
 
+// pool.queue[q] for a q known only at run time, as selects over the kernel parameter: indexing the parameter's array
+// directly copies the whole WfPool to every thread's stack at kernel entry.  The empty asm hides each entry from the
+// compiler, which would otherwise fold the selects back into that indexed load.
+__device__ __forceinline__ int *wfQueue(const WfPool &pool, int q) {
+    int *list = pool.queue[0];
+#pragma unroll
+    for (int k = 1; k < WQ_COUNT; ++k) {
+        int *entry = pool.queue[k];
+        asm("" : "+l"(entry));
+        list = q == k ? entry : list;
+    }
+    return list;
+}
+
 // warp-aggregated append of one index per participating lane
 __device__ __forceinline__ void wfPush(int *queue, unsigned *counter, int value, bool participate) {
     unsigned mask = __ballot_sync(0xffffffffu, participate);
@@ -136,17 +150,22 @@ __device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfP
 // Contexts on the free list take their next sample.  (Not inside k_wf_advance: there the few lanes of a warp that end a
 // path would run this code alone inside the register-heavy, low-occupancy shade kernel.)
 // GENERAL = true: the instantiation that can also draw from the SobolSampler (frames that use it).
+// The scene and the frame's parameters come as objects in device memory (renderWavefront uploads them once per render):
+// a struct passed by value whose address reaches a device function is copied to every thread's stack at kernel entry.
 template <bool GENERAL>
-__global__ void __launch_bounds__(256) k_wf_gen(DRenderParams rp, WfPool pool, int freeQ, int traceQ) {
+__global__ void __launch_bounds__(256) k_wf_gen(const DRenderParams *__restrict__ rpp, WfPool pool, int freeQ, int traceQ) {
+    const DRenderParams &rp = *rpp;
+    const int *freeList = wfQueue(pool, freeQ);
+    int *traceList = wfQueue(pool, traceQ);
     const unsigned n = pool.counts[freeQ];
     unsigned stride = gridDim.x * blockDim.x;
     unsigned cameraRays = 0;
     for (unsigned base = blockIdx.x * blockDim.x; base < n; base += stride) {
         unsigned i = base + threadIdx.x;
         const bool have = i < n;
-        const int c = have ? pool.queue[freeQ][i] : -1;
+        const int c = have ? freeList[i] : -1;
         const bool started = wfStartSample<GENERAL>(rp, pool, c, have, &cameraRays);
-        wfPush(pool.queue[traceQ], &pool.counts[traceQ], c, started);
+        wfPush(traceList, &pool.counts[traceQ], c, started);
     }
     for (int o = 16; o > 0; o >>= 1) cameraRays += __shfl_down_sync(0xffffffffu, cameraRays, o);
     if ((threadIdx.x & 31) == 0 && cameraRays) {
@@ -1107,15 +1126,19 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool p
 // TEX = true: the shade step of a scene with image textures (the camera ray's differentials are rebuilt from the
 // context's pFilm); one instantiation, with everything else compiled in.
 template <bool SHADE, bool SPH, int MINB, bool SPEC = false, bool LAZY = false, bool TEX = false>
-__global__ void __launch_bounds__(128, MINB) k_wf_advance(DScene sc, DRenderParams rp, WfPool pool, int srcQ, int traceQ,
-                                                                   int freeQ, float4 *film, unsigned long long *counters) {
+__global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool,
+                                                          int srcQ, int traceQ, int freeQ, float4 *film, unsigned long long *counters) {
+    const DScene &sc = *scp;
+    const DRenderParams &rp = *rpp;
+    const int *srcList = wfQueue(pool, srcQ);
+    int *traceList = wfQueue(pool, traceQ), *freeList = wfQueue(pool, freeQ);
     unsigned n = pool.counts[srcQ];
     unsigned stride = gridDim.x * blockDim.x;
     unsigned regular = 0, shadow = 0;
     for (unsigned base = blockIdx.x * blockDim.x; base < n; base += stride) {
         unsigned i = base + threadIdx.x;
         bool have = i < n;
-        int c = have ? pool.queue[srcQ][i] : 0;
+        int c = have ? srcList[i] : 0;
         bool ended = false, deferred = false;
         if (have) {
             WfCtx &cx = pool.ctx[c];
@@ -1149,8 +1172,8 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(DScene sc, DRenderPara
             }
         }
         if (SHADE && LAZY) wfPush(pool.queue[WQ_RETRY], &pool.counts[WQ_RETRY], c, deferred);
-        wfPush(pool.queue[traceQ], &pool.counts[traceQ], c, have && !ended && !deferred);
-        wfPush(pool.queue[freeQ], &pool.counts[freeQ], c, have && ended);
+        wfPush(traceList, &pool.counts[traceQ], c, have && !ended && !deferred);
+        wfPush(freeList, &pool.counts[freeQ], c, have && ended);
     }
     wfCountRays(counters, regular, shadow);
 }
@@ -1171,12 +1194,16 @@ __device__ __forceinline__ bool wfFinishNow(const DRenderParams &rp, const WfPoo
 }
 
 template <bool SPH, bool SPEC>
-__global__ void __launch_bounds__(128) k_wf_finish(DScene sc, DRenderParams rp, WfPool pool, int traceQ, unsigned threshold, float4 *film) {
+__global__ void __launch_bounds__(128) k_wf_finish(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool, int traceQ,
+                                                   unsigned threshold, float4 *film) {
+    const DScene &sc = *scp;
+    const DRenderParams &rp = *rpp;
     if (!wfFinishNow(rp, pool, traceQ, threshold)) return;
     const unsigned n = pool.counts[traceQ];
+    const int *traceList = wfQueue(pool, traceQ);
     unsigned regular = 0, shadow = 0;
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        WfCtx &cx = pool.ctx[pool.queue[traceQ][i]];
+        WfCtx &cx = pool.ctx[traceList[i]];
         DLane &ln = cx.ln;
         while (ln.state != LS_IDLE) {
             DHit hit;
