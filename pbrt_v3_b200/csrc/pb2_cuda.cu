@@ -1140,7 +1140,7 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
                 nLaunch += 3;
             }
             if (finishThreshold) finish<<<finishBlocks, 128, 0, st>>>(dSc, dRp, pool, WQ_TRACE0 + next, finishThreshold, film);
-            k_wf_reset<<<1, 32, 0, st>>>(rp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur, WQ_TRACE0 + next, finishThreshold);
+            k_wf_reset<<<1, 32, 0, st>>>(pool, WQ_FREE0 + cur, WQ_TRACE0 + cur, WQ_TRACE0 + next, finishThreshold);
             nLaunch += finishThreshold ? 6 : 5;
         }
         cur = next;

@@ -36,6 +36,9 @@ static_assert(offsetof(WfCtx, tHit) % 8 == 0 && offsetof(WfCtx, found) == offset
 
 // WQ_RETRY: path vertices deferred by the shade step (lazy light distribution), shaded again after k_lightdist_build
 enum { WQ_TRACE0 = 0, WQ_TRACE1 = 1, WQ_SHADE = 2, WQ_LIGHT = 3, WQ_FREE0 = 4, WQ_FREE1 = 5, WQ_CURSOR = 6, WQ_RETRY = 7, WQ_COUNT = 8 };
+// WQ_FINISH: the counter that holds k_wf_finish's decision of the round (0 = not taken yet), read by k_wf_reset.  It is
+// WQ_RETRY's: frames with a tail kernel are never lazily lit, so their retry list is never used.
+enum { WQ_FINISH = WQ_RETRY, WF_FINISH_WAIT = 1, WF_FINISH_GO = 2 };
 
 struct WfPool {
     int capacity;
@@ -97,14 +100,21 @@ struct WfChain {
 // MIS ray: add the BSDF sample if it reached the light), then the vertex's next ray - the MIS ray, or the continuation of
 // the path - or the end of the path (the sample goes to the film).  Returns the lane's new state.  Out of line: the
 // traversal loop must not carry its registers.
+// The hit is the one the trace kernel has just stored in the context ((leaf, b0, b1, b2), tHit, the found code), decoded
+// as k_wf_advance does: a MIS ray that reaches a one-sided area light is counted only when the light's surface at the
+// hit faces the ray, and a triangle's surface is built from the hit's barycentrics (its shading normals) and instance.
 template <bool SPH>
 __device__ __noinline__ int wfChainLight(const WfChain &ch, WfCtx *cx, bool found) {
     DLane &ln = cx->ln;
+    const float4 h4 = cx->hit;
+    const int foundCode = cx->found;
     DHit hit;
-    hit.leaf = __float_as_int(cx->hit.x);   // (meaningful for a MIS ray that hit something: the kernel stored it there)
-    hit.b0 = hit.b1 = hit.b2 = 0;
-    hit.inst = -1;
-    lightAdvance<SPH>(*ch.sc, ln, found, hit, 0.f);
+    hit.leaf = __float_as_int(h4.x);
+    hit.b0 = h4.y;
+    hit.b1 = h4.z;
+    hit.b2 = h4.w;
+    hit.inst = foundCode >= 2 ? foundCode - 2 : -1;
+    lightAdvance<SPH>(*ch.sc, ln, found, hit, cx->tHit);
     if (ln.state == LS_IDLE) addSample(*ch.rp, ch.film, cx->pFilm, guardRadiance(ln.L));
     return ln.state;
 }
@@ -1186,7 +1196,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
 // most `threshold` contexts are still in flight; then every thread takes ONE of them and walks it to the end of its
 // path with the per-lane state machine (traceLane + laneAdvance, the code of k_li_samples / pb2_li_samples), deposits
 // the sample, and the frame is over.  Same functions, same order of operations per path as the wavefront kernels.
-// k_wf_reset (below) empties the list under the same condition.
+// k_wf_reset (below) empties the list when k_wf_finish has walked it.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool wfFinishNow(const DRenderParams &rp, const WfPool &pool, int traceQ, unsigned threshold) {
     const unsigned n = pool.counts[traceQ];
@@ -1198,7 +1208,18 @@ __global__ void __launch_bounds__(128) k_wf_finish(const DScene *__restrict__ sc
                                                    unsigned threshold, float4 *film) {
     const DScene &sc = *scp;
     const DRenderParams &rp = *rpp;
-    if (!wfFinishNow(rp, pool, traceQ, threshold)) return;
+    // One decision for the whole launch and for this round's k_wf_reset.  The work counter is shared by the pipelines: it
+    // can run out while the blocks of this launch look at it, so each block deciding for itself could walk some of the
+    // listed paths and not others, and k_wf_reset could then empty a list whose paths were never walked.  The first block
+    // to look decides; the others and k_wf_reset follow it.
+    __shared__ bool sGo;
+    if (threadIdx.x == 0) {
+        const unsigned mine = wfFinishNow(rp, pool, traceQ, threshold) ? WF_FINISH_GO : WF_FINISH_WAIT;
+        const unsigned first = atomicCAS(&pool.counts[WQ_FINISH], 0u, mine);
+        sGo = (first ? first : mine) == WF_FINISH_GO;
+    }
+    __syncthreads();
+    if (!sGo) return;
     const unsigned n = pool.counts[traceQ];
     const int *traceList = wfQueue(pool, traceQ);
     unsigned regular = 0, shadow = 0;
@@ -1267,10 +1288,10 @@ __global__ void k_wf_init(WfPool pool) {
 }
 
 // end of a round: the lists consumed in it are emptied (and the next trace list, if k_wf_finish has just run it dry)
-__global__ void k_wf_reset(DRenderParams rp, WfPool pool, int a, int b, int traceNext, unsigned threshold) {
+__global__ void k_wf_reset(WfPool pool, int a, int b, int traceNext, unsigned threshold) {
     if (threadIdx.x == 0) {
-        pool.counts[WQ_RETRY] = 0;
-        if (wfFinishNow(rp, pool, traceNext, threshold)) pool.counts[traceNext] = 0;
+        if (threshold && pool.counts[WQ_FINISH] == WF_FINISH_GO) pool.counts[traceNext] = 0;
+        pool.counts[WQ_RETRY] = 0;   // (and WQ_FINISH)
         pool.counts[WQ_CURSOR] = 0;
         pool.counts[WQ_SHADE] = 0;
         pool.counts[WQ_LIGHT] = 0;

@@ -45,4 +45,6 @@ def work_items(film, params, tile_rank=0, tile_count=1):
     check(L.pb2_work_items(film, C.byref(p), 0, 0, None, C.byref(n)))
     out = np.zeros((n.value, 3), np.int32)
     check(L.pb2_work_items(film, C.byref(p), 0, n.value, ptr(out), None))
-    return out[out[:, 0] >= 0]
+    # a skipped item is (-1, -1, -1); a pixel coordinate alone may be negative (filters wider than a pixel extend the sample
+    # bounds beyond the film), a sample number never is
+    return out[out[:, 2] >= 0]

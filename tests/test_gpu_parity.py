@@ -266,7 +266,9 @@ def test_traversal_counters_equal_the_reference_order(pb, port):
     film2, st2 = hs.render_rgbw()
     assert np.allclose(film, film2, rtol=1e-5, atol=1e-5)
     assert st2.regular_rays == st.regular_rays and st2.shadow_rays == st.shadow_rays
-    # ... and so do the other kernels (two-child records, the 32-byte LinearBVHNode array, the small-stack builds)
+    # ... and so do the other kernels (two-child records, the 32-byte LinearBVHNode array, the small-stack builds).  At this
+    # size k_wf_finish takes over after round 0, so they trace camera rays only; test_gpu_wavefront_schedules.py renders
+    # them with the rounds forced
     for kname, flags in wf_kernels(pb).items():
         film3 = np.zeros((27, 48, 4), np.float32)
         st3 = pb.Stats()
@@ -598,8 +600,9 @@ def test_alpha_masked_meshes_through_every_render_kernel(pb):
 
 @pytest.mark.parametrize("name", ["soup", "materials", "instances", "specular", "lights"])
 def test_chained_light_step_renders_the_same_film(pb, name):
-    """PB2_FLAG_CHAIN (the light step inside the trace kernel: shadow ray, MIS ray and continuation follow each other in one
-    launch) changes the schedule, not the arithmetic of a path: same ray counts, same film up to the order of the atomic adds."""
+    """PB2_FLAG_CHAIN selects the chained trace kernel and the render still gives the same film and ray counts.  These scenes
+    are small enough for k_wf_finish to take over after round 0, before any shadow or MIS ray is in a trace list, so the
+    chained light step itself hardly runs here: test_gpu_wavefront_schedules.py checks it with the rounds forced."""
     hs = load_scene(pb, name)
     base, st0 = hs.render_rgbw(hs.params_copy(flags=0))
     film, st = hs.render_rgbw(hs.params_copy(flags=pb.PB2_FLAG_CHAIN))
