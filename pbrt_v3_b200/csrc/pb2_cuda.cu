@@ -1052,7 +1052,8 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         chain.film = film;
     }
     const bool spheres = scene->d.spheres != nullptr;
-    AdvanceKernel advLight = spheres ? k_wf_advance<false, true, 8> : k_wf_advance<false, false, 8>;
+    // light step: 7 resident blocks, as many as the shared-memory stage leaves room for (29 KB per block)
+    AdvanceKernel advLight = spheres ? k_wf_advance<false, true, 7> : k_wf_advance<false, false, 7>;
     AdvanceKernel advShade = scene->hasSpecular ? (spheres ? k_wf_advance<true, true, 4, true> : k_wf_advance<true, false, 4, true>)
                              : spheres ? k_wf_advance<true, true, 4>
                                        : k_wf_advance<true, false, 4>;
@@ -1099,7 +1100,6 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     const int capP = pools[0].capacity;
     // The list kernels' grid-stride grids stay oversubscribed: grids of resident size (SMs x occupancy) for gen, light and
     // shade were not faster on C2 (173.5 against 173.9 Msamples/s, medians of three, H100 80GB HBM3 at 700 W)
-    const int blocks256 = std::min((capP + 255) / 256, g_numSMs * 16);
     const int blocks128 = std::min((capP + 127) / 128, g_numSMs * 32);
     for (int p = 0; p < nPipes; ++p) k_wf_init<<<(capP + 255) / 256, 256, 0, streams[p]>>>(pools[p]);
     unsigned long long nLaunch = nPipes;
@@ -1112,8 +1112,8 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         for (int p = 0; p < nPipes; ++p) {
             const WfPool &pool = pools[p];
             cudaStream_t st = streams[p];
-            if (sobol) k_wf_gen<true><<<blocks256, 256, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
-            else k_wf_gen<false><<<blocks256, 256, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
+            if (sobol) k_wf_gen<true><<<blocks128, 128, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
+            else k_wf_gen<false><<<blocks128, 128, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
             if (timeTrace) {
                 if (scene->traceEvents.size() < nEvents + 2) {
                     cudaEvent_t e0, e1;

@@ -33,6 +33,102 @@ struct alignas(32) WfCtx {
 static_assert(offsetof(WfCtx, ln) == 0 && offsetof(DLane, state) == 0 && offsetof(DLane, ray) == 4 && sizeof(DRay) == 28,
               "the trace kernels read the first 32 bytes of a context as {state, o, d, tMax}");
 static_assert(offsetof(WfCtx, tHit) % 8 == 0 && offsetof(WfCtx, found) == offsetof(WfCtx, tHit) + 4, "tHit/found are stored as one float2");
+static_assert(sizeof(DLane) == 192 && offsetof(WfCtx, hit) == 192 && offsetof(WfCtx, tHit) == 208 && offsetof(WfCtx, pFilm) == 216 &&
+                  sizeof(WfCtx) == 224 && sizeof(WfCtx) % 32 == 0,
+              "a context is seven whole 32-byte sectors: the lane (six), then hit, tHit / found and pFilm (one)");
+
+// ---------------------------------------------------------------------------------------------
+// The list kernels (gen, light step, shade step) do not work on a context in place.  The 32 lanes of a warp hold 32
+// unrelated contexts, so every scalar field access would be an instruction that touches 32 sectors of HBM, and every
+// store of 4-12 bytes would leave a partial sector in L2.  Instead the warp copies its 32 contexts into shared memory with
+// 16-byte streaming loads (each instruction: 512 contiguous bytes of ~2.3 contexts, every fetched sector used whole),
+// each thread works on its copy, and the warp writes back the sectors the kernel can change with 16-byte streaming
+// stores.  Streaming (evict-first) because a context is touched once per kernel: the BVH, which the other pipeline's
+// trace launch is reading at the same time, should keep the L2.
+// ---------------------------------------------------------------------------------------------
+// A context in shared memory: WfCtx's bytes, padded from 224 to 232.  At 56 words per slot the 32 lanes of a warp
+// reach 4 of the 32 banks with a 4-byte access (8-way conflicts); at 58 words, 16 with a 4-byte access and all 32 with
+// an 8-byte one.
+struct WfSlot {
+    DLane ln;
+    float hit[4];   // (leaf record, b0, b1, b2)
+    float tHit;
+    int found;
+    V2 pFilm;
+    int pad[2];
+};
+static_assert(offsetof(WfSlot, hit) == offsetof(WfCtx, hit) && offsetof(WfSlot, tHit) == offsetof(WfCtx, tHit) &&
+                  offsetof(WfSlot, found) == offsetof(WfCtx, found) && offsetof(WfSlot, pFilm) == offsetof(WfCtx, pFilm) &&
+                  sizeof(WfSlot) == 232 && alignof(WfSlot) == 8,
+              "a slot holds a context's bytes at the context's offsets, 8-byte aligned, 58 words apart");
+
+// Bytes at the start of a lane that a kernel can change and writes back (whole sectors):
+//   WF_OUT_START  k_wf_gen: laneStartPath sets every field before lightNum; lightNum and pick (the rest of the third
+//                 sector) are set by the shade step before anything reads them
+//   WF_OUT_LIGHT  k_wf_advance<light>: lightAdvance changes state, ray, L, beta, bounces and ldSum, all below misTerm
+//   WF_OUT_SHADE  k_wf_advance<shade>: the whole lane
+enum { WF_OUT_START = 96, WF_OUT_LIGHT = 128, WF_OUT_SHADE = (int)sizeof(DLane) };
+static_assert(offsetof(DLane, lightNum) == 88 && offsetof(DLane, pick) == 92 && offsetof(DLane, ldSum) == 96 && offsetof(DLane, ldLight) == 108 &&
+                  offsetof(DLane, bounces) < 96 && offsetof(DLane, misTerm) == 120,
+              "the written-back prefixes above cover the fields their kernels change");
+
+// The lane index, read anew at every call: derived from threadIdx, the chunk addresses of the copies below are loop
+// invariants of a list kernel's grid-stride loop, and the compiler hoists all ~50 of them out of it (the shade step then
+// spills ~500 bytes).
+__device__ __forceinline__ int wfLaneId() {
+    int lane;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+    return lane;
+}
+
+// Warp-collective (all 32 lanes, converged): lane l's context c (c < 0: none) is copied into warpSlots[l].  Two batches
+// of seven 16-byte loads per lane, all of a batch in flight at once.
+__device__ __forceinline__ void wfStageIn(const WfCtx *ctx, WfSlot *warpSlots, int c) {
+    constexpr int CHUNKS = sizeof(WfCtx) / 16, BATCH = CHUNKS / 2;
+    const int lane = wfLaneId();
+    __syncwarp();
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+        uint4 v[BATCH];
+        int cs[BATCH];
+#pragma unroll
+        for (int it = 0; it < BATCH; ++it) {
+            const int q = (b * BATCH + it) * 32 + lane, j = q / CHUNKS, k = q % CHUNKS;
+            cs[it] = __shfl_sync(0xffffffffu, c, j);
+            if (cs[it] >= 0) v[it] = __ldcs(reinterpret_cast<const uint4 *>(ctx + cs[it]) + k);
+        }
+#pragma unroll
+        for (int it = 0; it < BATCH; ++it) {
+            const int q = (b * BATCH + it) * 32 + lane, j = q / CHUNKS, k = q % CHUNKS;
+            if (cs[it] >= 0) {
+                uint2 *s = reinterpret_cast<uint2 *>(reinterpret_cast<char *>(&warpSlots[j]) + 16 * k);
+                s[0] = make_uint2(v[it].x, v[it].y);
+                s[1] = make_uint2(v[it].z, v[it].w);
+            }
+        }
+    }
+    __syncwarp();
+}
+
+// Warp-collective: the first BYTES bytes of lane l's slot go back to its context c (c < 0: none).
+template <int BYTES>
+__device__ __forceinline__ void wfStageOut(WfCtx *ctx, const WfSlot *warpSlots, int c) {
+    static_assert(BYTES % 32 == 0 && BYTES <= (int)sizeof(DLane), "whole sectors of the lane");
+    constexpr int CHUNKS = BYTES / 16;
+    const int lane = wfLaneId();
+    __syncwarp();
+#pragma unroll
+    for (int it = 0; it < CHUNKS; ++it) {
+        const int q = it * 32 + lane, j = q / CHUNKS, k = q % CHUNKS;
+        const int cj = __shfl_sync(0xffffffffu, c, j);
+        if (cj >= 0) {
+            const uint2 *s = reinterpret_cast<const uint2 *>(reinterpret_cast<const char *>(&warpSlots[j]) + 16 * k);
+            const uint2 lo = s[0], hi = s[1];
+            __stcs(reinterpret_cast<uint4 *>(ctx + cj) + k, make_uint4(lo.x, lo.y, hi.x, hi.y));
+        }
+    }
+    __syncwarp();
+}
 
 // WQ_RETRY: path vertices deferred by the shade step (lazy light distribution), shaded again after k_lightdist_build
 enum { WQ_TRACE0 = 0, WQ_TRACE1 = 1, WQ_SHADE = 2, WQ_LIGHT = 3, WQ_FREE0 = 4, WQ_FREE1 = 5, WQ_CURSOR = 6, WQ_RETRY = 7, WQ_COUNT = 8 };
@@ -123,8 +219,9 @@ __device__ __noinline__ int wfChainLight(const WfChain &ch, WfCtx *cx, bool foun
 // (Halton dims 0-4, perspective camera).  Warp-collective: all 32 lanes call it, `want` says which of them take part; work
 // items that map outside the sample bounds / pixel bounds are skipped (integrator.cpp:274), so a lane may draw several.
 // Returns false for a lane that did not want a sample or found the work counter exhausted (its context retires).
+// The new lane and pFilm are built in `slot`.
 template <bool GENERAL>
-__device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfPool &pool, int c, bool want, unsigned *cameraRays) {
+__device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfPool &pool, WfSlot &slot, bool want, unsigned *cameraRays) {
     bool started = false;
     while (__any_sync(0xffffffffu, want && !started)) {
         const bool draw = want && !started;
@@ -140,14 +237,13 @@ __device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfP
             } else {
                 int px, py, sample;
                 if (decodeWork(rp, item, &px, &py, &sample)) {
-                    WfCtx &cx = pool.ctx[c];
                     DSampler smp;
                     smp.index = sampleIndex<GENERAL>(rp.halton, px, py, sample);
                     smp.dim = 0;
                     V2 pFilm;
                     DRay ray = generateCameraRay<GENERAL>(rp.cam, rp.halton, smp, px, py, &pFilm);
-                    laneStartPath(cx.ln, ray, smp);
-                    cx.pFilm = pFilm;
+                    laneStartPath(slot.ln, ray, smp);
+                    slot.pFilm = pFilm;
                     ++*cameraRays;
                     started = true;
                 }
@@ -162,8 +258,12 @@ __device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfP
 // GENERAL = true: the instantiation that can also draw from the SobolSampler (frames that use it).
 // The scene and the frame's parameters come as objects in device memory (renderWavefront uploads them once per render):
 // a struct passed by value whose address reaches a device function is copied to every thread's stack at kernel entry.
+// The new lanes are built in shared memory and written out as whole sectors (WF_OUT_START), pFilm as one 8-byte store.
 template <bool GENERAL>
-__global__ void __launch_bounds__(256) k_wf_gen(const DRenderParams *__restrict__ rpp, WfPool pool, int freeQ, int traceQ) {
+__global__ void __launch_bounds__(128) k_wf_gen(const DRenderParams *__restrict__ rpp, WfPool pool, int freeQ, int traceQ) {
+    __shared__ WfSlot stage[128];
+    WfSlot &slot = stage[threadIdx.x];
+    WfSlot *warpSlots = stage + (threadIdx.x & ~31u);
     const DRenderParams &rp = *rpp;
     const int *freeList = wfQueue(pool, freeQ);
     int *traceList = wfQueue(pool, traceQ);
@@ -174,7 +274,13 @@ __global__ void __launch_bounds__(256) k_wf_gen(const DRenderParams *__restrict_
         unsigned i = base + threadIdx.x;
         const bool have = i < n;
         const int c = have ? freeList[i] : -1;
-        const bool started = wfStartSample<GENERAL>(rp, pool, c, have, &cameraRays);
+        const bool started = wfStartSample<GENERAL>(rp, pool, slot, have, &cameraRays);
+        if (started) {
+            slot.ln.lightNum = 0;   // (not read before the shade step sets them: written only to store no stale shared memory)
+            slot.ln.pick = 0;
+            __stcs(reinterpret_cast<float2 *>(&pool.ctx[c].pFilm), make_float2(slot.pFilm.x, slot.pFilm.y));
+        }
+        wfStageOut<WF_OUT_START>(pool.ctx, warpSlots, started ? c : -1);
         wfPush(traceList, &pool.counts[traceQ], c, started);
     }
     for (int o = 16; o > 0; o >>= 1) cameraRays += __shfl_down_sync(0xffffffffu, cameraRays, o);
@@ -1138,6 +1244,9 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool p
 template <bool SHADE, bool SPH, int MINB, bool SPEC = false, bool LAZY = false, bool TEX = false>
 __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool,
                                                           int srcQ, int traceQ, int freeQ, float4 *film, unsigned long long *counters) {
+    __shared__ WfSlot stage[128];
+    WfSlot &slot = stage[threadIdx.x];
+    WfSlot *warpSlots = stage + (threadIdx.x & ~31u);
     const DScene &sc = *scp;
     const DRenderParams &rp = *rpp;
     const int *srcList = wfQueue(pool, srcQ);
@@ -1150,23 +1259,22 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
         bool have = i < n;
         int c = have ? srcList[i] : 0;
         bool ended = false, deferred = false;
+        wfStageIn(pool.ctx, warpSlots, have ? c : -1);
         if (have) {
-            WfCtx &cx = pool.ctx[c];
-            DLane &ln = cx.ln;  // updated in place: each kernel touches only the fields its state needs
-            const float4 h4 = cx.hit;
-            const int foundCode = cx.found;
+            DLane &ln = slot.ln;
+            const int foundCode = slot.found;
             DHit hit;
-            hit.leaf = __float_as_int(h4.x);
-            hit.b0 = h4.y;
-            hit.b1 = h4.z;
-            hit.b2 = h4.w;
+            hit.leaf = __float_as_int(slot.hit[0]);
+            hit.b0 = slot.hit[1];
+            hit.b1 = slot.hit[2];
+            hit.b2 = slot.hit[3];
             hit.inst = foundCode >= 2 ? foundCode - 2 : -1;
             bool found = foundCode != 0;
-            float tHit = cx.tHit;
+            float tHit = slot.tHit;
             if (SHADE && TEX) {
                 DTexCtx tc;
                 tc.cam = &rp.cam;
-                tc.pFilm = cx.pFilm;
+                tc.pFilm = slot.pFilm;
                 tc.diffScale = rp.diffScale;
                 shadeVertex<SPH, SPEC, LAZY, true>(sc, rp.halton, rp.path, ln, found, hit, tHit, &tc);
             } else if (SHADE) shadeVertex<SPH, SPEC, LAZY>(sc, rp.halton, rp.path, ln, found, hit, tHit);
@@ -1176,11 +1284,13 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
                 deferred = true;
             } else {
                 ended = ln.state == LS_IDLE;
-                if (ended) addSample(rp, film, cx.pFilm, guardRadiance(ln.L));
+                if (ended) addSample(rp, film, slot.pFilm, guardRadiance(ln.L));
                 else if (ln.state == LS_SHADOW) shadow++;   // Scene::IntersectP call (scene.cpp:51-55)
                 else regular++;                             // Scene::Intersect call (scene.cpp:45-49)
             }
         }
+        // (an ended path's lane is not written back: its context goes to the free list, and k_wf_gen starts a new lane in it)
+        wfStageOut<SHADE ? WF_OUT_SHADE : WF_OUT_LIGHT>(pool.ctx, warpSlots, have && !ended ? c : -1);
         if (SHADE && LAZY) wfPush(pool.queue[WQ_RETRY], &pool.counts[WQ_RETRY], c, deferred);
         wfPush(traceList, &pool.counts[traceQ], c, have && !ended && !deferred);
         wfPush(freeList, &pool.counts[freeQ], c, have && ended);
