@@ -95,9 +95,15 @@ struct DTexCtx {
     float diffScale;    // 1 / sqrt(samples per pixel)
 };
 
+// u: room for the vertex's kSampleBatch sampler values (the caller's: shared memory in the shade step).
 template <bool SPH, bool SPEC = true, bool LAZY = true, bool TEX = false>
 PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &pp, DLane &ln, bool found, const DHit &hit,
-                        float tMax, const DTexCtx *tc = nullptr) {
+                        float tMax, float *u, const DTexCtx *tc = nullptr) {
+    // Every dimension this vertex can draw, [smp.dim, smp.dim + kSampleBatch), evaluated up front: the values are a pure
+    // function of (index, dimension), and drawn here their table loads overlap the hit's leaf-record loads instead of
+    // forming a chain of round trips each where its value is used.  A vertex that draws nothing skips it.
+    const int dim0 = ln.smp.dim;
+    if (found && ln.bounces < pp.maxDepth) haltonSampleBatch<TEX>(h, ln.smp.index, dim0, kSampleBatch, u);
     DInteraction isect;
     int li = -1;
     DTexGeom tg;
@@ -168,14 +174,14 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
     if (ln.doNEE && sc.nLights > 0) {
         // UniformSampleOneLight (integrator.cpp:85-106)
         float lightPickPdf;
-        int lightNum = sampleDiscrete(distrib, sc.nLights, get1D<TEX>(h, smp), &lightPickPdf);
+        int lightNum = sampleDiscrete(distrib, sc.nLights, get1D<TEX>(h, smp, u, dim0), &lightPickPdf);
         if (lightPickPdf != 0) {
             ln.pick = lightPickPdf;
             ln.lightNum = lightNum;
             const pb2_light light = sc.lights[lightNum];
             const TriRec lightRec = loadTriRec(sc.lightRecs, (size_t)lightNum);
-            V2 uLight = get2D<TEX>(h, smp);
-            V2 uScattering = get2D<TEX>(h, smp);
+            V2 uLight = get2D<TEX>(h, smp, u, dim0);
+            V2 uScattering = get2D<TEX>(h, smp, u, dim0);
             // EstimateDirect, light-sampling half (integrator.cpp:116-160)
             DLightSample ls = sampleLight<SPH>(sc, lightNum, light, lightRec, isect, uLight);
             float lightPdf = ls.pdf, scatteringPdf = 0;
@@ -225,7 +231,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
         V3 wo = -ln.ray.d, wi;
         float pdf;
         int sampled = 0;
-        V3 f = bsdfSampleF<SPEC>(bsdf, wo, &wi, get2D<TEX>(h, smp), &pdf, &sampled);
+        V3 f = bsdfSampleF<SPEC>(bsdf, wo, &wi, get2D<TEX>(h, smp, u, dim0), &pdf, &sampled);
         if (!(isBlack(f) || pdf == 0.f)) {
             V3 s = f * absDot(wi, isect.ns);
             V3 beta = ln.beta * mk3(s.x / pdf, s.y / pdf, s.z / pdf);
@@ -240,7 +246,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             V3 rrBeta = beta * ln.etaScale;
             if (maxComponentValue(rrBeta) < pp.rrThreshold && ln.bounces > 3) {
                 float q = pmax(.05f, 1 - maxComponentValue(rrBeta));
-                if (get1D<TEX>(h, smp) < q) survive = false;
+                if (get1D<TEX>(h, smp, u, dim0) < q) survive = false;
                 else {
                     float d = 1 - q;
                     beta = mk3(beta.x / d, beta.y / d, beta.z / d);
@@ -296,8 +302,11 @@ PB2_HD void lightAdvance(const DScene &sc, DLane &ln, bool found, const DHit &hi
 template <bool SPH, bool SPEC = true, bool TEX = false>
 PB2_HD bool laneAdvance(const DScene &sc, const DHalton &h, const DPathParams &pp, DLane &ln, bool found, const DHit &hit,
                         float tMax, const DTexCtx *tc = nullptr) {
-    if (ln.state == LS_PATH) shadeVertex<SPH, SPEC, true, TEX>(sc, h, pp, ln, found, hit, tMax, tc);
-    else lightAdvance<SPH>(sc, ln, found, hit, tMax);
+    if (ln.state == LS_PATH) {
+        float u[kSampleBatch];
+        shadeVertex<SPH, SPEC, true, TEX>(sc, h, pp, ln, found, hit, tMax, u, tc);
+    } else
+        lightAdvance<SPH>(sc, ln, found, hit, tMax);
     return ln.state == LS_IDLE;
 }
 

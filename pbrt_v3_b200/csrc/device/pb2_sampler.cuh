@@ -241,6 +241,16 @@ PB2_HD float haltonSample(const DHalton &h, int64_t index, int dim) {
 #endif
 }
 
+// A read of table data that never changes during a kernel: through the read-only data cache on the device.
+template <class T>
+PB2_HD T ldTab(const T *p) {
+#if defined(__CUDA_ARCH__)
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+
 // SobolIntervalToIndex (lowdiscrepancy.h:229-249): the index of sample `frame` of pixel p (relative to the sample bounds)
 PB2_HD uint64_t sobolIntervalToIndex(const DHalton &h, uint64_t frame, int px, int py) {
     const uint32_t m = (uint32_t)h.sobolLog2Res;
@@ -279,6 +289,90 @@ PB2_HD float sampleDimension(const DHalton &h, int64_t index, int dim) {
     return haltonSample(h, index, dim);
 }
 
+// The dimensions a path vertex can draw (light pick 1, uLight 2, uScattering 2, continuation 2, Russian roulette 1)
+constexpr int kSampleBatch = 8;
+
+// sampleDimension<GENERAL>(h, index, dim0 + k) for k < n <= kSampleBatch, bit for bit.  Every value is a pure function of (index,
+// dimension), so all of a vertex's dimensions can be evaluated as soon as the vertex starts.  Drawn one at a time, each is a
+// chain of dependent loads (dimension record, table header, nat / full, pow / invPow); here the loads of all n dimensions
+// go out in three waves - every table header, then every nat / full entry, then every pow / invPow - so a vertex waits
+// for about three round trips instead of three or four per dimension.  Each element is scrambledRadicalInverseTab's integer
+// arithmetic and float operations.  Dimensions 0 and 1, indices of 2^32 and above, the digit-loop build (no tables) and the
+// SobolSampler take sampleDimension per element.
+template <bool GENERAL = false>
+PB2_HD void haltonSampleBatch(const DHalton &h, int64_t index, int dim0, int n, float *out) {
+#if defined(__CUDACC__)
+    if (!(GENERAL && h.sobol) && h.dimTabs && dim0 >= 2 && dim0 + n <= kMaxHaltonDims && ((uint64_t)index >> 32) == 0) {
+        const uint32_t a = (uint32_t)index;
+        uint4 hdr[kSampleBatch];        // HaltonDimTab's {magicB (two words), B, m}
+        uint32_t off[kSampleBatch];     // HaltonDimTab::tabOffset
+#pragma unroll
+        for (int k = 0; k < kSampleBatch; ++k) {
+            if (k < n) {
+                const HaltonDimTab *t = h.dimTabs + dim0 + k;
+                hdr[k] = ldTab(reinterpret_cast<const uint4 *>(t));
+                off[k] = ldTab(&t->tabOffset);
+            }
+        }
+        uint32_t q2[kSampleBatch], lo16[kSampleBatch], mid16[kSampleBatch];
+#pragma unroll
+        for (int k = 0; k < kSampleBatch; ++k) {
+            if (k < n) {
+                const uint64_t magicB = (uint64_t)hdr[k].x | ((uint64_t)hdr[k].y << 32);
+                const uint32_t B = hdr[k].z;
+                const uint16_t *nat = h.digitTab + off[k], *full = nat + B;
+                const uint32_t q1 = divMagic(a, magicB), lo = a - q1 * B;
+                if (q1 == 0) {
+                    lo16[k] = ldTab(nat + lo);
+                    q2[k] = 0;
+                    mid16[k] = 0xffffffffu;   // no second block
+                } else {
+                    const uint32_t q = divMagic(q1, magicB), mid = q1 - q * B;
+                    lo16[k] = ldTab(full + lo);
+                    mid16[k] = q == 0 ? ldTab(nat + mid) : ldTab(full + mid);
+                    q2[k] = q;
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < kSampleBatch; ++k) {
+            if (k < n) {
+                const HaltonDimTab *t = h.dimTabs + dim0 + k;
+                const uint32_t B = hdr[k].z, m = hdr[k].w;
+                uint64_t reversedDigits;
+                uint32_t nd;
+                if (mid16[k] == 0xffffffffu) {
+                    const uint32_t e = lo16[k];
+                    reversedDigits = e & 0x1fffu;
+                    nd = e >> 13;
+                } else if (q2[k] == 0) {
+                    const uint32_t f = lo16[k], e = mid16[k], nh = e >> 13;
+                    reversedDigits = (uint64_t)f * ldTab(&t->pow[nh]) + (e & 0x1fffu);
+                    nd = m + nh;
+                } else {
+                    // an index of more than 2 m digits: the rest one digit at a time, as the loop would
+                    const ulonglong2 rec = ldTab(h.dimRecs + dim0 + k);   // {ceil(2^64 / prime), prime | primeSum << 32}
+                    const uint32_t base = (uint32_t)rec.y;
+                    const uint16_t *perm = h.perms + (uint32_t)(rec.y >> 32);
+                    reversedDigits = (uint64_t)lo16[k] * B + mid16[k];
+                    nd = 2 * m;
+                    uint32_t rest = q2[k];
+                    while (rest) {
+                        const uint32_t next = divMagic(rest, rec.x), digit = rest - next * base;
+                        reversedDigits = reversedDigits * base + ldTab(perm + digit);
+                        ++nd;
+                        rest = next;
+                    }
+                }
+                out[k] = pmin(ldTab(&t->invPow[nd]) * ((float)reversedDigits + ldTab(&t->tail)), kOneMinusEpsilon);
+            }
+        }
+        return;
+    }
+#endif
+    for (int k = 0; k < n; ++k) out[k] = sampleDimension<GENERAL>(h, index, dim0 + k);
+}
+
 // GlobalSampler::GetIndexForSample: HaltonSampler's (halton.cpp:96-116) or SobolSampler's (sobol.cpp:41-44)
 template <bool GENERAL>
 PB2_HD int64_t sampleIndex(const DHalton &h, int px, int py, int64_t sampleNum) {
@@ -299,6 +393,22 @@ PB2_HD V2 get2D(const DHalton &h, DSampler &s) {
     V2 p = mk2(sampleDimension<GENERAL>(h, s.index, s.dim), sampleDimension<GENERAL>(h, s.index, s.dim + 1));
     s.dim += 2;
     return p;
+}
+
+// The same draws from a vertex's batch (haltonSampleBatch): u[k] holds dimension dim0 + k.  A dimension past the batch is
+// evaluated directly; the counter moves as above.
+template <bool GENERAL = false>
+PB2_HD float get1D(const DHalton &h, DSampler &s, const float *u, int dim0) {
+    const int k = s.dim - dim0;
+    const float v = k < kSampleBatch ? u[k] : sampleDimension<GENERAL>(h, s.index, s.dim);
+    s.dim++;
+    return v;
+}
+template <bool GENERAL = false>
+PB2_HD V2 get2D(const DHalton &h, DSampler &s, const float *u, int dim0) {
+    const float x = get1D<GENERAL>(h, s, u, dim0);
+    const float y = get1D<GENERAL>(h, s, u, dim0);
+    return mk2(x, y);
 }
 
 // sampling.cpp:113-130

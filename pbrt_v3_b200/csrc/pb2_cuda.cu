@@ -725,6 +725,17 @@ __global__ void k_halton_samples(DHalton h, const int32_t *pixelXY, const int64_
     else out[i] = sampleDimension<true>(h, index, dim[i]);
 }
 
+// the sampler batch of the shade step (haltonSampleBatch) for explicit (pixel, sample, first dimension) triples
+__global__ void k_halton_batch(DHalton h, const int32_t *pixelXY, const int64_t *sampleNum, const int32_t *dim0, int64_t n, float *out) {
+    int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t index = sampleIndex<true>(h, pixelXY[2 * i], pixelXY[2 * i + 1], sampleNum[i]);
+    float u[kSampleBatch];
+    haltonSampleBatch<true>(h, index, dim0[i], kSampleBatch, u);
+#pragma unroll
+    for (int k = 0; k < kSampleBatch; ++k) out[kSampleBatch * i + k] = u[k];
+}
+
 __global__ void k_light_distribution(DScene sc, const float *points, int64_t n, float *out) {
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -1296,6 +1307,70 @@ int pb2_debug_radical_inverse_tables(const uint32_t *index, const int32_t *dim, 
         out_loop[i] = scrambledRadicalInverse32(base, magic, index[i], perm);
         out_tab[i] = scrambledRadicalInverseTab(g_halton.hDimTabs[dim[i]], g_halton.hDigitTab.data(), base, magic, index[i], perm);
     }
+    return PB2_OK;
+}
+
+// Host-side check of the shade step's sampler batch (tests, no device): with the host tables, haltonSampleBatch of
+// index[i] over dimensions dim0[i] .. dim0[i] + 7 (out_batch, 8 per item) and scrambledRadicalInverseTab of each of those
+// dimensions (out_tab); the two must agree bit for bit.  The film and parameters give the DHalton a render would use.
+int pb2_debug_halton_batch(const pb2_film_desc *film, const pb2_path_params *pp, const uint32_t *index, const int32_t *dim0, int64_t n,
+                           float *out_batch, float *out_tab) {
+    if (!film || !pp || !index || !dim0 || !out_batch || !out_tab) return setError(PB2_ERR_INVALID, "null argument");
+    buildHaltonHostTables();
+    DHalton h = makeHalton(film, pp);
+    h.perms = g_halton.hPerms.data();
+    h.primes = g_halton.hPrimes.data();
+    h.primeSums = g_halton.hPrimeSums.data();
+    h.dimRecs = g_halton.hDimRecs.data();
+    h.dimTabs = g_halton.hDimTabs.data();
+    h.digitTab = g_halton.hDigitTab.data();
+    for (int64_t i = 0; i < n; ++i) {
+        if (dim0[i] < 2 || dim0[i] + kSampleBatch > kMaxHaltonDims) return setError(PB2_ERR_INVALID, "dimension out of range");
+        haltonSampleBatch(h, (int64_t)index[i], dim0[i], kSampleBatch, out_batch + kSampleBatch * i);
+        for (int k = 0; k < kSampleBatch; ++k) {
+            const int d = dim0[i] + k;
+            const uint32_t base = (uint32_t)g_halton.hPrimes[d];
+            const uint16_t *perm = g_halton.hPerms.data() + g_halton.hPrimeSums[d];
+            out_tab[kSampleBatch * i + k] = scrambledRadicalInverseTab(g_halton.hDimTabs[d], g_halton.hDigitTab.data(), base,
+                                                                       g_halton.hDimRecs[d].x, index[i], perm);
+        }
+    }
+    return PB2_OK;
+}
+
+// Device-side check of the same batch: for each (pixel, sample number) the sample's index as a render computes it, then
+// haltonSampleBatch over dimensions dim0[i] .. dim0[i] + 7 on the device (8 values per item in out), to be compared with
+// pb2_halton_samples of the same dimensions.
+int pb2_debug_halton_batch_device(const pb2_film_desc *film, const pb2_path_params *pp, const int32_t *pixel_xy,
+                                  const int64_t *sample_num, const int32_t *dim0, int64_t n, float *out) {
+    int rc = requireDevice();
+    if (rc) return rc;
+    if (!film || !pp || (n > 0 && (!pixel_xy || !sample_num || !dim0 || !out))) return setError(PB2_ERR_INVALID, "null argument");
+    if (n <= 0) return PB2_OK;
+    for (int64_t i = 0; i < n; ++i)
+        if (dim0[i] < 0 || dim0[i] + kSampleBatch > kMaxHaltonDims) return setError(PB2_ERR_INVALID, "dimension out of range");
+    DHalton h = makeHalton(film, pp);
+    if (pp->sampler == PB2_SAMPLER_SOBOL && (rc = attachSobol(&h, film))) return rc;
+    int32_t *dXY = nullptr, *dDim = nullptr;
+    int64_t *dS = nullptr;
+    float *dOut = nullptr;
+    cudaError_t e = cudaMalloc((void **)&dXY, n * 2 * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc((void **)&dS, n * sizeof(int64_t));
+    if (e == cudaSuccess) e = cudaMalloc((void **)&dDim, n * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc((void **)&dOut, n * kSampleBatch * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemcpy(dXY, pixel_xy, n * 2 * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dS, sample_num, n * sizeof(int64_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dDim, dim0, n * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+        k_halton_batch<<<(unsigned)((n + 127) / 128), 128>>>(h, dXY, dS, dDim, n, dOut);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out, dOut, n * kSampleBatch * sizeof(float), cudaMemcpyDeviceToHost);
+    cudaFree(dXY);
+    cudaFree(dS);
+    cudaFree(dDim);
+    cudaFree(dOut);
+    if (e != cudaSuccess) return setError(PB2_ERR_CUDA, std::string("pb2_debug_halton_batch_device: ") + cudaGetErrorString(e));
     return PB2_OK;
 }
 

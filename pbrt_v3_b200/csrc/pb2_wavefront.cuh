@@ -1245,8 +1245,12 @@ template <bool SHADE, bool SPH, int MINB, bool SPEC = false, bool LAZY = false, 
 __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool,
                                                           int srcQ, int traceQ, int freeQ, float4 *film, unsigned long long *counters) {
     __shared__ WfSlot stage[128];
+    // the shade step's sampler batch (shadeVertex): one row per thread, padded to 9 words so that a warp's 32 rows fall
+    // in 32 different banks
+    __shared__ float sampleRows[SHADE ? 128 * (kSampleBatch + 1) : 1];
     WfSlot &slot = stage[threadIdx.x];
     WfSlot *warpSlots = stage + (threadIdx.x & ~31u);
+    float *u = sampleRows + (SHADE ? threadIdx.x * (kSampleBatch + 1) : 0);
     const DScene &sc = *scp;
     const DRenderParams &rp = *rpp;
     const int *srcList = wfQueue(pool, srcQ);
@@ -1276,8 +1280,8 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
                 tc.cam = &rp.cam;
                 tc.pFilm = slot.pFilm;
                 tc.diffScale = rp.diffScale;
-                shadeVertex<SPH, SPEC, LAZY, true>(sc, rp.halton, rp.path, ln, found, hit, tHit, &tc);
-            } else if (SHADE) shadeVertex<SPH, SPEC, LAZY>(sc, rp.halton, rp.path, ln, found, hit, tHit);
+                shadeVertex<SPH, SPEC, LAZY, true>(sc, rp.halton, rp.path, ln, found, hit, tHit, u, &tc);
+            } else if (SHADE) shadeVertex<SPH, SPEC, LAZY>(sc, rp.halton, rp.path, ln, found, hit, tHit, u);
             else lightAdvance<SPH>(sc, ln, found, hit, tHit);
             if (SHADE && LAZY && ln.state == LS_DEFER) {
                 ln.state = LS_PATH;   // untouched: shaded again from the retry list once its voxel's record exists
