@@ -8,6 +8,7 @@ Both export the same entry points (prefix ``ref_`` / ``orc_``) over the same ``p
 library consumes.  Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
 legs may import this module; the product (pbrt_v3_b200/) never does.
 """
+import contextlib
 import ctypes as C
 import os
 
@@ -141,6 +142,44 @@ class Oracle:
         k = np.zeros(3, np.float32)
         self._f("copper_rgb")(ptr(eta), ptr(k))
         return eta, k
+
+    @property
+    def has_device_math(self):
+        """True when this library was linked by oracle/Makefile.ref with the device-math wrappers (a reference library built
+        by an older recipe has neither the wrappers nor the switch)."""
+        return self.kind == "reference" and hasattr(self.L, "ref_set_device_math") and hasattr(self.L, "__wrap_sinf")
+
+    @contextlib.contextmanager
+    def device_math(self, on=True):
+        """Within the block the reference evaluates sinf / cosf / sincosf / logf / atan2f / acosf as the device does,
+        (float)f((double)x) (oracle/ref_devmath.cpp), while it traces, samples, shades and looks textures up; scenes, lights,
+        films, cameras and textures are still built with glibc's functions.  The previous setting is restored on exit
+        (reference only: the port has no such switch)."""
+        if self.kind != "reference":
+            raise RuntimeError("device math is a mode of the compiled reference, not of the %s oracle" % self.kind)
+        if not self.has_device_math:
+            raise RuntimeError("%s was built without the device-math wrappers: rebuild it with oracle/Makefile.ref" % self.L._name)
+        fn = self._f("set_device_math")
+        fn.argtypes, fn.restype = [C.c_int], C.c_int
+        was = fn(1 if on else 0)
+        try:
+            yield self
+        finally:
+            fn(was)
+
+    TRANSCENDENTALS = {"sinf": 0, "cosf": 1, "sincosf": 2, "logf": 3, "atan2f": 4, "acosf": 5}
+
+    def transcendental(self, name, a, b=None):
+        """One of the six wrapped float functions, called from the reference's harness under the current device-math setting:
+        (n,) results, (n, 2) = (sin, cos) for sincosf; atan2f takes y = a, x = b (reference only)."""
+        a = np.ascontiguousarray(a, np.float32)
+        b = np.ascontiguousarray(a if b is None else b, np.float32)
+        out = np.zeros((len(a), 2) if name == "sincosf" else len(a), np.float32)
+        fn = self._f("transcendentals")
+        fn.argtypes = [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
+        if fn(self.TRANSCENDENTALS[name], len(a), ptr(a), ptr(b), ptr(out)):
+            raise ValueError(name)
+        return out
 
     def transform(self, kind, args):
         args = np.ascontiguousarray(args, np.float32)

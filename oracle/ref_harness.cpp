@@ -131,7 +131,23 @@ struct LinearBVHNode {
 
 using namespace pbrt;
 
+// Device math.  libpbrt_ref.so routes the reference's sinf / cosf / sincosf / logf / atan2f / acosf through
+// ref_devmath.cpp, which computes them as the device does while ref_devmath_active is set.  ref_set_device_math(1) makes
+// the entry points below set it around evaluation only (tracing, sampling, Li, look-ups), never while scenes, lights,
+// films, cameras or textures are built: the tables those constructors fill (MIPMap's Lanczos weights, the infinite light's
+// Distribution2D, the sinc filter's table) are built by the library on the host with glibc, as here.  The spatial light
+// distribution, which the reference fills lazily during Li, is evaluation; the device builds it with its own functions.
+// libb200_overlay.so includes this file but links glibc's functions directly, so the flag changes nothing there.
+std::atomic<int> ref_devmath_active{0};
+
 namespace {
+
+int g_deviceMathMode = 0;
+
+struct DeviceMathScope {
+    DeviceMathScope() { ref_devmath_active.store(g_deviceMathMode); }
+    ~DeviceMathScope() { ref_devmath_active.store(0); }
+};
 
 struct RefScene {
     std::vector<std::unique_ptr<Transform>> transforms;
@@ -336,6 +352,31 @@ extern "C" {
 
 const char *ref_kind(void) { return "reference"; }
 
+// Device math for the evaluation entry points (see DeviceMathScope); returns the previous setting
+int ref_set_device_math(int on) {
+    const int was = g_deviceMathMode;
+    g_deviceMathMode = on != 0;
+    return was;
+}
+
+// The six wrapped functions as the reference's own code calls them, under the current device-math setting.
+// fn: 0 sinf, 1 cosf, 2 sincosf (sin, cos per element), 3 logf, 4 atan2f(y = a, x = b), 5 acosf.
+int ref_transcendentals(int fn, int64_t n, const float *a, const float *b, float *out) {
+    DeviceMathScope dm;
+    for (int64_t i = 0; i < n; ++i) {
+        switch (fn) {
+        case 0: out[i] = sinf(a[i]); break;
+        case 1: out[i] = cosf(a[i]); break;
+        case 2: sincosf(a[i], &out[2 * i], &out[2 * i + 1]); break;
+        case 3: out[i] = logf(a[i]); break;
+        case 4: out[i] = atan2f(a[i], b[i]); break;
+        case 5: out[i] = acosf(a[i]); break;
+        default: return 1;
+        }
+    }
+    return 0;
+}
+
 // MIPMap<T>::pyramid[level] of the reference for one texture description (row-major, channels floats per texel)
 int ref_texture_pyramid(const pb2_texture *t, int level, int *n_levels, int *w, int *h, float *out) {
     setThreads(0);
@@ -404,6 +445,7 @@ int ref_texture_lookup(const pb2_texture *t, int64_t n, const float *st, const f
     const size_t nt = (size_t)t->width * t->height;
     if (t->channels == 1) {
         MIPMap<Float> mm(Point2i(t->width, t->height), t->texels, t->do_trilinear != 0, t->max_anisotropy, wrap);
+        DeviceMathScope dm;
         for (int64_t i = 0; i < n; ++i) {
             Float v = mm.Lookup(Point2f(st[2 * i], st[2 * i + 1]), Vector2f(dst[4 * i], dst[4 * i + 1]), Vector2f(dst[4 * i + 2], dst[4 * i + 3]));
             out[3 * i] = out[3 * i + 1] = out[3 * i + 2] = v;
@@ -412,6 +454,7 @@ int ref_texture_lookup(const pb2_texture *t, int64_t n, const float *st, const f
         std::vector<RGBSpectrum> texels(nt);
         for (size_t i = 0; i < nt; ++i) texels[i] = RGBSpectrum::FromRGB(t->texels + 3 * i);
         MIPMap<RGBSpectrum> mm(Point2i(t->width, t->height), texels.data(), t->do_trilinear != 0, t->max_anisotropy, wrap);
+        DeviceMathScope dm;
         for (int64_t i = 0; i < n; ++i)
             mm.Lookup(Point2f(st[2 * i], st[2 * i + 1]), Vector2f(dst[4 * i], dst[4 * i + 1]), Vector2f(dst[4 * i + 2], dst[4 * i + 3])).ToRGB(out + 3 * i);
     }
@@ -427,6 +470,7 @@ int ref_texture_evaluate(const pb2_texture *textures, int n_textures, int id, in
     std::vector<std::shared_ptr<Texture<Float>>> floatTex;
     std::vector<std::shared_ptr<Texture<Spectrum>>> specTex;
     buildRefTextures(&d, floatTex, specTex);
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         SurfaceInteraction si;
         si.uv = Point2f(uv[2 * i], uv[2 * i + 1]);
@@ -449,6 +493,7 @@ int ref_bsdf_eval(const pb2_material *pm, int64_t n, const float *in, float *out
     std::shared_ptr<Material> material = makeRefMaterial(*pm, floatTex, specTex);
     MemoryArena arena;
     const BxDFType nonSpecular = BxDFType(BSDF_ALL & ~BSDF_SPECULAR);
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         const float *q = in + 17 * i;
         float *o = out + 19 * i;
@@ -669,6 +714,7 @@ int64_t ref_bvh_dump(void *h, pb2_bvh_node *out_nodes, int64_t max_nodes, int32_
 
 int ref_intersect(void *h, const pb2_ray *rays, int64_t n, pb2_hit *hits) {
     RefScene *rs = static_cast<RefScene *>(h);
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         Ray ray(Point3f(rays[i].o[0], rays[i].o[1], rays[i].o[2]), Vector3f(rays[i].d[0], rays[i].d[1], rays[i].d[2]),
                 rays[i].t_max);
@@ -699,6 +745,7 @@ int ref_intersect(void *h, const pb2_ray *rays, int64_t n, pb2_hit *hits) {
 
 int ref_intersect_p(void *h, const pb2_ray *rays, int64_t n, uint8_t *occluded) {
     RefScene *rs = static_cast<RefScene *>(h);
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         Ray ray(Point3f(rays[i].o[0], rays[i].o[1], rays[i].o[2]), Vector3f(rays[i].d[0], rays[i].d[1], rays[i].d[2]),
                 rays[i].t_max);
@@ -717,7 +764,10 @@ int ref_render(void *h, const pb2_camera *cam, const pb2_film_desc *fd, const pb
     ReportThreadStats();  // flush this thread's counters from earlier calls, then start from zero
     ClearStats();
     auto t0 = std::chrono::steady_clock::now();
-    ro.integrator->Render(*rs->scene);
+    {
+        DeviceMathScope dm;
+        ro.integrator->Render(*rs->scene);
+    }
     auto t1 = std::chrono::steady_clock::now();
     if (seconds) *seconds = std::chrono::duration<double>(t1 - t0).count();
     {
@@ -752,6 +802,7 @@ int ref_li_samples(void *h, const pb2_camera *cam, const pb2_film_desc *fd, cons
     ro.integrator->Preprocess(*rs->scene, *ro.sampler);
     MemoryArena arena;
     std::unique_ptr<Sampler> sampler = ro.sampler->Clone(0);
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         Point2i pixel(pixel_xy[2 * i], pixel_xy[2 * i + 1]);
         sampler->StartPixel(pixel);
@@ -787,6 +838,7 @@ int ref_camera_differentials(void *h, const pb2_camera *cam, const pb2_film_desc
     setThreads(1);
     RenderObjects ro = makeRenderObjects(*rs, cam, fd, pp);
     std::unique_ptr<Sampler> sampler = ro.sampler->Clone(0);
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         float *o = out + 39 * i;
         std::memset(o, 0, 39 * sizeof(float));
@@ -820,6 +872,7 @@ int ref_halton_samples(const pb2_film_desc *fd, const pb2_path_params *pp, const
                         (int)std::floor(fd->cropped_pixel_bounds[1] + 0.5f - fd->filter_radius[1])),
                 Point2i((int)std::ceil(fd->cropped_pixel_bounds[2] - 0.5f + fd->filter_radius[0]),
                         (int)std::ceil(fd->cropped_pixel_bounds[3] - 0.5f + fd->filter_radius[1])));
+    DeviceMathScope dm;
     if (pp->sampler == PB2_SAMPLER_SOBOL) {
         SobolSampler ss(pp->samples_per_pixel, sb);
         for (int64_t i = 0; i < n; ++i) {
@@ -867,6 +920,7 @@ int ref_light_distribution(void *h, const float *points, int64_t n, float *out) 
     RefScene *rs = static_cast<RefScene *>(h);
     if (!rs->distrib) rs->distrib = CreateLightSampleDistribution(strategyName(rs->lightStrategy), *rs->scene);
     size_t nl = rs->lights.size(), stride = 2 * nl + 1;
+    DeviceMathScope dm;
     for (int64_t i = 0; i < n; ++i) {
         const Distribution1D *d = rs->distrib->Lookup(Point3f(points[3 * i], points[3 * i + 1], points[3 * i + 2]));
         for (size_t k = 0; k < nl; ++k) out[i * stride + k] = d->func[k];

@@ -52,6 +52,27 @@ def bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
+def row_digest(a):
+    """A 32-bit digest of every bit of each row of an array of 4-byte values (FNV-1a over the words, folded): fixtures keep
+    these instead of the values where the values would make them large."""
+    w = np.ascontiguousarray(a).view(np.uint32).reshape(len(a), -1).astype(np.uint64)
+    h = np.full(len(a), 0xcbf29ce484222325, np.uint64)
+    for j in range(w.shape[1]):
+        h = (h ^ w[:, j]) * np.uint64(0x100000001b3)
+    return (h ^ (h >> np.uint64(32))).astype(np.uint32)
+
+
+def pixel_digests(items, li, pfilm):
+    """Per pixel of the work items (x, y, sample): the pixels in sorted order and a digest of every bit of every sample's
+    sample number, L and pFilm there."""
+    rows = np.concatenate([np.ascontiguousarray(items[:, 2:3], np.int32).view(np.float32), np.asarray(li, np.float32),
+                           np.asarray(pfilm, np.float32)], 1)
+    pixels, inv = np.unique(np.asarray(items[:, :2], np.int32), axis=0, return_inverse=True)
+    acc = np.zeros(len(pixels), np.uint64)
+    np.add.at(acc, inv.ravel(), row_digest(rows).astype(np.uint64))
+    return pixels, (acc ^ (acc >> np.uint64(32))).astype(np.uint32)
+
+
 # Reconstruction filters (src/filters/): the PixelFilter line and the Film line of each case; geometry, lights and
 # materials are tests/scenes/materials.pbrt's.  Wider-than-a-pixel filters make neighbouring tiles overlap in the film,
 # so the order in which tiles are merged shows in the last bit: these cases are rendered by ONE thread on the CPU side.

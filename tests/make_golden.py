@@ -259,6 +259,10 @@ def main():
     record_openexr_images(ref_dir)
     record_filters(ref)
     record_hlbvh(ref)
+    # the reference in device-math mode, for tests/test_gpu_exact_parity.py
+    import test_gpu_exact_parity
+    test_gpu_exact_parity.record_reference(ref, os.path.join(OUT, "exact_parity.npz"))
+    print("exact parity fixture written")
     # the metal material's default eta / k: copper's measured spectra through Spectrum::FromSampled (metal.cpp:121-126)
     eta, k = ref.copper_rgb()
     np.savez_compressed(os.path.join(OUT, "metal_defaults.npz"), eta=eta, k=k)

@@ -8,6 +8,11 @@ Tolerances (also stated in DESIGN.md):
     sampled direction can flip an edge decision or move a sharp microfacet lobe).
   * images: >= 99.9 % of the pixels within 1 % relative, mean relative error <= 1e-4, image mean within 1e-4.
   * Scene::Intersect / IntersectP call counters: equal to the reference's within 0.1 % (edge flips).
+These pin the device to the glibc goldens and to the port.  The transcendentals are the only reason for them:
+test_gpu_exact_parity.py runs the compiled reference with the device's definitions of sinf / cosf / sincosf / logf / atan2f /
+acosf and asserts per-sample Li, every hit field, look-ups, light distributions and ray counters EQUAL, and films within the
+float32 summation bound of the reference's samples.  Measured effect (test_ref_device_math.py): the device's definitions
+change Li in 1032 of the 57 000 golden samples (1 to 445 of 3000 per scene, most on the environment-lit scenes).
 """
 import ctypes as C
 import os
