@@ -425,6 +425,13 @@ int pb2_host_free(void *p);
  * tables (src/core/lightdistrib.cpp:232-300) on the device. */
 int pb2_scene_create(const pb2_scene_desc *desc, pb2_scene **out);
 int pb2_scene_destroy(pb2_scene *scene);
+/* The shade feature class pb2_scene_create gives the scene described by desc (host only, no device needed): a bit
+ * mask of what the scene's material and light records can produce, 1 = an Oren-Nayar lobe (matte, sigma != 0),
+ * 2 = a plastic Trowbridge-Reitz lobe, 4 = a point, spot, distant or infinite light; 7 when a specular-family material
+ * (mirror, glass, substrate, metal, uber) is present or the environment sets PB2_SHADE_GENERAL=1.  A scene of class 0
+ * (Lambertian surfaces lit by area lights) gets a shade step compiled for that class alone, unless it also has spheres,
+ * image textures, the SobolSampler or the lazily built light distribution. */
+int pb2_shade_class(const pb2_scene_desc *desc, int32_t *out);
 
 /* Scene::Intersect for a batch of rays (src/core/scene.cpp:45-49). rays/hits are HOST pointers. */
 int pb2_intersect(pb2_scene *scene, const pb2_ray *rays, int64_t n, pb2_hit *hits);

@@ -96,7 +96,8 @@ struct DTexCtx {
 };
 
 // u: room for the vertex's kSampleBatch sampler values (the caller's: shared memory in the shade step).
-template <bool SPH, bool SPEC = true, bool LAZY = true, bool TEX = false>
+// FC: the scene's shade feature class (SHADE_* in pb2_shade.cuh), SHADE_ALL when it is not known.
+template <bool SPH, bool SPEC = true, bool LAZY = true, bool TEX = false, int FC = SHADE_ALL>
 PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &pp, DLane &ln, bool found, const DHit &hit,
                         float tMax, float *u, const DTexCtx *tc = nullptr) {
     // Every dimension this vertex can draw, [smp.dim, smp.dim + kSampleBatch), evaluated up front: the values are a pure
@@ -144,8 +145,9 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             if (li >= 0) ln.L = ln.L + ln.beta * lightL(sc.lights[li], isect.n, -ln.ray.d);
         } else {
             // the ray escaped: every infinite light is seen directly (path.cpp:96-98)
-            for (int k = 0; k < sc.nInfinite; ++k)
-                ln.L = ln.L + ln.beta * infiniteLe(sc, sc.lights[sc.infinite[k]], sc.deltaLights[sc.infinite[k]], ln.ray.d);
+            if (FC & SHADE_NON_AREA)
+                for (int k = 0; k < sc.nInfinite; ++k)
+                    ln.L = ln.L + ln.beta * infiniteLe(sc, sc.lights[sc.infinite[k]], sc.deltaLights[sc.infinite[k]], ln.ray.d);
         }
     }
     if (!found || ln.bounces >= pp.maxDepth) {
@@ -154,7 +156,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
     }
     if (TEX) ln.camRay = false;   // every ray spawned from here on is a plain Ray
     DBsdf bsdf;
-    if (!makeBsdf<SPEC, TEX>(sc, isect, &bsdf, TEX ? &uvDiff : nullptr)) {
+    if (!makeBsdf<SPEC, TEX, FC>(sc, isect, &bsdf, TEX ? &uvDiff : nullptr)) {
         ln.ray = spawnRay(isect, ln.ray.d);  // null BSDF: skip the surface, same bounce count
         return;
     }
@@ -183,11 +185,11 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             V2 uLight = get2D<TEX>(h, smp, u, dim0);
             V2 uScattering = get2D<TEX>(h, smp, u, dim0);
             // EstimateDirect, light-sampling half (integrator.cpp:116-160)
-            DLightSample ls = sampleLight<SPH>(sc, lightNum, light, lightRec, isect, uLight);
+            DLightSample ls = sampleLight<SPH, FC>(sc, lightNum, light, lightRec, isect, uLight);
             float lightPdf = ls.pdf, scatteringPdf = 0;
             if (lightPdf > 0 && !isBlack(ls.Li)) {
-                V3 f = bsdfF<SPEC>(bsdf, isect.wo, ls.wi) * absDot(ls.wi, isect.ns);
-                scatteringPdf = bsdfPdf<SPEC>(bsdf, isect.wo, ls.wi);
+                V3 f = bsdfF<SPEC, FC>(bsdf, isect.wo, ls.wi) * absDot(ls.wi, isect.ns);
+                scatteringPdf = bsdfPdf<SPEC, FC>(bsdf, isect.wo, ls.wi);
                 if (!isBlack(f)) {
                     shadow = spawnRayTo(isect, ls.p, ls.pError, ls.n);
                     hasShadow = true;
@@ -201,19 +203,19 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             V3 wi;
             V3 f = mk3(0, 0, 0);
             if (!ls.delta) {
-                f = bsdfSampleF<SPEC>(bsdf, isect.wo, &wi, uScattering, &scatteringPdf, nullptr, true);
+                f = bsdfSampleF<SPEC, FC>(bsdf, isect.wo, &wi, uScattering, &scatteringPdf, nullptr, true);
                 if (scatteringPdf != 0) f = f * absDot(wi, isect.ns);
                 else f = mk3(0, 0, 0);
             }
             if (!isBlack(f) && scatteringPdf > 0) {
-                lightPdf = lightPdfLi<SPH>(sc, light, lightRec, isect, wi, lightNum);
+                lightPdf = lightPdfLi<SPH, FC>(sc, light, lightRec, isect, wi, lightNum);
                 if (lightPdf != 0) {
                     float weight = powerHeuristic(scatteringPdf, lightPdf);
                     // Li is the light's Lemit when the MIS ray reaches its emitting side (checked after
                     // the trace); f * Li * Tr(=1) * weight / scatteringPdf.  An infinite light is seen when the ray
                     // escapes instead (integrator.cpp:209-211): its Le along wi is known here already.
                     V3 Lmis = mk3(light.L[0], light.L[1], light.L[2]);
-                    if (sc.deltaLights && light.type == PB2_LIGHT_INFINITE) Lmis = infiniteLe(sc, light, sc.deltaLights[lightNum], wi);
+                    if ((FC & SHADE_NON_AREA) && sc.deltaLights && light.type == PB2_LIGHT_INFINITE) Lmis = infiniteLe(sc, light, sc.deltaLights[lightNum], wi);
                     V3 fl = f * Lmis * weight;
                     ln.misTerm = mk3(fl.x / scatteringPdf, fl.y / scatteringPdf, fl.z / scatteringPdf);
                     DRay mr = spawnRay(isect, wi);
@@ -231,7 +233,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
         V3 wo = -ln.ray.d, wi;
         float pdf;
         int sampled = 0;
-        V3 f = bsdfSampleF<SPEC>(bsdf, wo, &wi, get2D<TEX>(h, smp, u, dim0), &pdf, &sampled);
+        V3 f = bsdfSampleF<SPEC, FC>(bsdf, wo, &wi, get2D<TEX>(h, smp, u, dim0), &pdf, &sampled);
         if (!(isBlack(f) || pdf == 0.f)) {
             V3 s = f * absDot(wi, isect.ns);
             V3 beta = ln.beta * mk3(s.x / pdf, s.y / pdf, s.z / pdf);
@@ -269,16 +271,17 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
 }
 
 // A shadow or MIS ray has been traced: add its term, then start the vertex's next ray or finish it.
-template <bool SPH>
+template <bool SPH, int FC = SHADE_ALL>
 PB2_HD void lightAdvance(const DScene &sc, DLane &ln, bool found, const DHit &hit, float tMax) {
+    const bool nonArea = (FC & SHADE_NON_AREA) && sc.deltaLights;
     if (ln.state == LS_SHADOW) {
         if (!found) ln.ldSum = ln.ldSum + ln.ldLight;  // VisibilityTester::Unoccluded
         startMisOrFinish(ln);
     } else {
         if (!found) {
             // the MIS ray escaped: Li = light.Le(ray), which is zero for every light but an infinite one (integrator.cpp:209-211)
-            if (sc.deltaLights && sc.lights[ln.lightNum].type == PB2_LIGHT_INFINITE) ln.ldSum = ln.ldSum + ln.misTerm;
-        } else if (!(sc.deltaLights && sc.lights[ln.lightNum].type == PB2_LIGHT_INFINITE)) {
+            if (nonArea && sc.lights[ln.lightNum].type == PB2_LIGHT_INFINITE) ln.ldSum = ln.ldSum + ln.misTerm;
+        } else if (!(nonArea && sc.lights[ln.lightNum].type == PB2_LIGHT_INFINITE)) {
             // the hit primitive's light number rides in its leaf record (spheres: via primLight)
             float4 b = ldg4(&sc.leafPrims[3 * (size_t)hit.leaf + 1]), c = ldg4(&sc.leafPrims[3 * (size_t)hit.leaf + 2]);
             int hitLight = asInt(c.w);
@@ -299,14 +302,14 @@ PB2_HD void lightAdvance(const DScene &sc, DLane &ln, bool found, const DHit &hi
 
 // Advance a lane after its current ray was traced.  Returns true when the path ended in this call
 // (ln.L is then final and ln.state == LS_IDLE).
-template <bool SPH, bool SPEC = true, bool TEX = false>
+template <bool SPH, bool SPEC = true, bool TEX = false, int FC = SHADE_ALL>
 PB2_HD bool laneAdvance(const DScene &sc, const DHalton &h, const DPathParams &pp, DLane &ln, bool found, const DHit &hit,
                         float tMax, const DTexCtx *tc = nullptr) {
     if (ln.state == LS_PATH) {
         float u[kSampleBatch];
-        shadeVertex<SPH, SPEC, true, TEX>(sc, h, pp, ln, found, hit, tMax, u, tc);
+        shadeVertex<SPH, SPEC, true, TEX, FC>(sc, h, pp, ln, found, hit, tMax, u, tc);
     } else
-        lightAdvance<SPH>(sc, ln, found, hit, tMax);
+        lightAdvance<SPH, FC>(sc, ln, found, hit, tMax);
     return ln.state == LS_IDLE;
 }
 

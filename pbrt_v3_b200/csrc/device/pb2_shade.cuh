@@ -289,6 +289,14 @@ struct DBsdf {
     float e;               // the index the lobes' Fresnel terms use (BSDF::eta is 1 when GEN_OPACITY is present)
 };
 enum { BSDF_SAMPLED_SPECULAR = 1, BSDF_SAMPLED_TRANSMISSION = 2 };
+// A shade feature class (the FC template argument of the BSDF, light and lane functions): the lobes and lights that the
+// scene's material and light records can produce among those of the non-specular materials' BSDFs and the area lights.
+// A bit that is clear compiles away a branch whose run-time condition is false for every record of such a scene; the
+// code that remains is the same, in the same order.  The host picks the class (shadeFeatureClass in pb2_cuda.cu).
+//   SHADE_OREN_NAYAR   a matte material with sigma != 0 (diffuseKind 2)
+//   SHADE_MICROFACET   a plastic material (its Trowbridge-Reitz lobe, hasMicrofacet)
+//   SHADE_NON_AREA     a point, spot, distant or infinite light (DScene::deltaLights, nInfinite)
+enum { SHADE_OREN_NAYAR = 1, SHADE_MICROFACET = 2, SHADE_NON_AREA = 4, SHADE_ALL = 7, SHADE_LAMBERT_AREA = 0 };
 enum { GEN_OPACITY = 1, GEN_LAMBERT = 2, GEN_MICROFACET = 4, GEN_SPEC_REFLECTION = 8, GEN_SPEC_TRANSMISSION = 16,
        GEN_MICRO_TRANSMISSION = 32,   // MicrofacetTransmission(specT, TrowbridgeReitz(alphaX, alphaY), 1, e): rough glass
        GEN_LOBES = 6, GEN_NON_SPECULAR = GEN_LAMBERT | GEN_MICROFACET | GEN_MICRO_TRANSMISSION };
@@ -356,7 +364,7 @@ PB2_HDN void bumpShading(const DScene &sc, int tex, const DTexGeom &tg, const DU
 }
 
 // TEX = true: image textures are evaluated (uvDiff: the point's (u, v) differentials); false compiles them away.
-template <bool SPEC = true, bool TEX = false>
+template <bool SPEC = true, bool TEX = false, int FC = SHADE_ALL>
 PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, const DUvDiff *uvDiff = nullptr) {
     int m = sc.primMaterial[it.prim];
     if (m < 0) return false;
@@ -511,7 +519,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         float sig = clampf(mat.sigma, 0.f, 90.f);
         if (!isBlack(kd)) {
             bsdf->R = kd;
-            if (sig == 0)
+            if (!(FC & SHADE_OREN_NAYAR) || sig == 0)
                 bsdf->diffuseKind = 1;
             else {
                 bsdf->diffuseKind = 2;
@@ -529,7 +537,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
             bsdf->nLobes++;
         }
         V3 ks = clampSpectrum(mat.ks);
-        if (!isBlack(ks)) {
+        if ((FC & SHADE_MICROFACET) && !isBlack(ks)) {
             float rough = mat.roughness;
             if (mat.remap_roughness) rough = roughnessToAlpha(rough);
             bsdf->Ks = ks;
@@ -706,8 +714,9 @@ PB2_HD float blendPdf(const DBsdf &b, V3 wo, V3 wi) {
 }
 
 // individual BxDFs (local frame)
+template <int FC = SHADE_ALL>
 PB2_HD V3 diffuseF(const DBsdf &b, V3 wo, V3 wi) {
-    if (b.diffuseKind == 1) return b.R * kInvPi;
+    if (!(FC & SHADE_OREN_NAYAR) || b.diffuseKind == 1) return b.R * kInvPi;
     // OrenNayar::f (reflection.cpp:197-219)
     float sinThetaI = sinTheta(wi), sinThetaO = sinTheta(wo);
     float maxCos = 0;
@@ -835,7 +844,7 @@ PB2_HD V3 genF(const DBsdf &b, V3 wo, V3 wi, bool reflect) {
 
 // BSDF::f (reflection.cpp:680-693).  All lobes in scope are reflective and non-specular, so they
 // match both BSDF_ALL and BSDF_ALL & ~BSDF_SPECULAR.
-template <bool SPEC = true>
+template <bool SPEC = true, int FC = SHADE_ALL>
 PB2_HD V3 bsdfF(const DBsdf &b, V3 woW, V3 wiW) {
     V3 wi = worldToLocal(b, wiW), wo = worldToLocal(b, woW);
     if (wo.z == 0) return mk3(0, 0, 0);
@@ -844,13 +853,13 @@ PB2_HD V3 bsdfF(const DBsdf &b, V3 woW, V3 wiW) {
     if (SPEC && b.blend) return reflect ? blendF(b, wo, wi) : f;
     if (SPEC && b.general) return genF(b, wo, wi, reflect);
     if (reflect) {
-        if (b.diffuseKind) f = f + diffuseF(b, wo, wi);
-        if (b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
+        if (b.diffuseKind) f = f + diffuseF<FC>(b, wo, wi);
+        if ((FC & SHADE_MICROFACET) && b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
     }
     return f;
 }
 // BSDF::Pdf (reflection.cpp:781-796)
-template <bool SPEC = true>
+template <bool SPEC = true, int FC = SHADE_ALL>
 PB2_HD float bsdfPdf(const DBsdf &b, V3 woW, V3 wiW) {
     if (b.nLobes == 0) return 0.f;
     V3 wo = worldToLocal(b, woW), wi = worldToLocal(b, wiW);
@@ -866,7 +875,7 @@ PB2_HD float bsdfPdf(const DBsdf &b, V3 woW, V3 wiW) {
     }
     float pdf = 0.f;
     if (b.diffuseKind) pdf += diffusePdf(wo, wi);
-    if (b.hasMicrofacet) pdf += microfacetPdf(b, wo, wi);
+    if ((FC & SHADE_MICROFACET) && b.hasMicrofacet) pdf += microfacetPdf(b, wo, wi);
     return pdf / b.nLobes;
 }
 // BSDF::Sample_f (reflection.cpp:714-779).  Returns f; *pdf == 0 means no sample.
@@ -966,7 +975,7 @@ PB2_HDN V3 genSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
 }
 
 // *sampledFlags (optional): BSDF_SAMPLED_* of the BxDF that was sampled.
-template <bool SPEC = true>
+template <bool SPEC = true, int FC = SHADE_ALL>
 PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sampledFlags = nullptr, bool nonSpecularOnly = false) {
     *pdf = 0;
     if (sampledFlags) *sampledFlags = 0;
@@ -1039,7 +1048,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     int comp = (int)floorf(u.x * matching);
     if (comp > matching - 1) comp = matching - 1;
     // lobe order: diffuse first, then microfacet (plastic.cpp:53-68)
-    bool sampleMicro = b.hasMicrofacet && (comp == matching - 1) && !(b.diffuseKind && comp == 0);
+    bool sampleMicro = (FC & SHADE_MICROFACET) && b.hasMicrofacet && (comp == matching - 1) && !(b.diffuseKind && comp == 0);
     V2 uRemapped = mk2(pmin(u.x * matching - comp, kOneMinusEpsilon), u.y);
     V3 wo = worldToLocal(b, woW), wi;
     if (wo.z == 0) return mk3(0, 0, 0);
@@ -1049,7 +1058,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
         wi = cosineSampleHemisphere(uRemapped);
         if (wo.z < 0) wi.z *= -1;
         *pdf = diffusePdf(wo, wi);
-        f = diffuseF(b, wo, wi);
+        f = diffuseF<FC>(b, wo, wi);
     } else {
         // MicrofacetReflection::Sample_f (reflection.cpp:410-423); wo.z == 0 handled above
         V3 wh = trSampleWh(b.alpha, wo, uRemapped);
@@ -1061,7 +1070,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     }
     if (*pdf == 0) return mk3(0, 0, 0);
     *wiW = localToWorld(b, wi);
-    if (matching > 1) {
+    if ((FC & SHADE_MICROFACET) && matching > 1) {   // (two lobes: plastic's)
         if (sampleMicro) *pdf += diffusePdf(wo, wi);
         else *pdf += microfacetPdf(b, wo, wi);
         *pdf /= matching;
@@ -1070,8 +1079,8 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     bool reflect = dot(*wiW, b.ng) * dot(woW, b.ng) > 0;
     f = mk3(0, 0, 0);
     if (reflect) {
-        if (b.diffuseKind) f = f + diffuseF(b, wo, wi);
-        if (b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
+        if (b.diffuseKind) f = f + diffuseF<FC>(b, wo, wi);
+        if ((FC & SHADE_MICROFACET) && b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
     }
     return f;
 }
@@ -1377,10 +1386,11 @@ PB2_HDN float infinitePdfLi(const DDeltaLight &dl, V3 w) {
 }
 
 // `rec` is the light's record out of DScene::lightRecs, lightNum its index in Scene::lights.
-template <bool SPH = true>
+template <bool SPH = true, int FC = SHADE_ALL>
 PB2_HD DLightSample sampleLight(const DScene &sc, int lightNum, const pb2_light &l, const TriRec &rec, const DInteraction &ref, V2 u) {
-    if (sc.deltaLights && l.type == PB2_LIGHT_INFINITE) return sampleInfiniteLight(sc, l, sc.deltaLights[lightNum], ref.p, u);
-    if (sc.deltaLights && l.type != PB2_LIGHT_AREA) return sampleDeltaLight(l, sc.deltaLights[lightNum], ref.p);
+    const bool nonArea = (FC & SHADE_NON_AREA) && sc.deltaLights;
+    if (nonArea && l.type == PB2_LIGHT_INFINITE) return sampleInfiniteLight(sc, l, sc.deltaLights[lightNum], ref.p, u);
+    if (nonArea && l.type != PB2_LIGHT_AREA) return sampleDeltaLight(l, sc.deltaLights[lightNum], ref.p);
     DLightSample s;
     if (SPH && (rec.flags & LEAF_SPHERE)) s = sampleSphereLight(sc, l, ref, u);
     else s = sampleTriangleLight(sc, l, rec, ref.p, u);
@@ -1390,9 +1400,9 @@ PB2_HD DLightSample sampleLight(const DScene &sc, int lightNum, const pb2_light 
 
 // DiffuseAreaLight::Pdf_Li -> Shape::Pdf(ref, wi) (shape.cpp:78-95): re-intersect the light's own
 // shape with the spawned ray and convert the area density to solid angle.
-template <bool SPH = true>
+template <bool SPH = true, int FC = SHADE_ALL>
 PB2_HD float lightPdfLi(const DScene &sc, const pb2_light &l, const TriRec &rec, const DInteraction &ref, V3 wi, int lightNum = -1) {
-    if (sc.deltaLights && l.type == PB2_LIGHT_INFINITE) return infinitePdfLi(sc.deltaLights[lightNum], wi);
+    if ((FC & SHADE_NON_AREA) && sc.deltaLights && l.type == PB2_LIGHT_INFINITE) return infinitePdfLi(sc.deltaLights[lightNum], wi);
     if (SPH && (rec.flags & LEAF_SPHERE)) return sphereLightPdf(sc, l, ref, wi);
     DRay ray = spawnRay(ref, wi);
     const TriVerts t = rec.tv;

@@ -401,6 +401,7 @@ struct pb2_scene {
     int bvhDepth = 0;  // maximum number of simultaneously pending far children = tree depth (scene BVH)
     int instDepth = 0; // the same for the deepest instanced object's BVH
     bool hasSpecular = false;  // a mirror / glass material exists: the shade kernel with the specular BxDFs is used
+    int shadeClass = SHADE_ALL;   // shadeFeatureClass: SHADE_LAMBERT_AREA selects the shade step compiled for that class
     int devIndex = 0;             // entry of g_devs this copy lives on
     std::vector<pb2_scene *> replicas;   // primary only: the copies on g_devs[1..] (pb2_init_devices with several devices)
     bool lazyLightDist = false;   // spatial light distribution built on demand (DLightDist::slots)
@@ -1036,6 +1037,9 @@ static WfPool poolOf(const pb2_scene *scene, int capacity, int pipe = 0, int nPi
     return pool;
 }
 
+// Resident blocks per SM of the SHADE_LAMBERT_AREA shade step (__launch_bounds__ minimum; DESIGN.md section 3)
+constexpr int kShadeLambertAreaMinBlocks = 4;
+
 // Host driver of the wavefront rounds (see pb2_wavefront.cuh).
 static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *film, cudaStream_t stream, int flags,
                            bool timeTrace, unsigned long long *launches, double *traceMs) {
@@ -1063,8 +1067,16 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         chain.film = film;
     }
     const bool spheres = scene->d.spheres != nullptr;
+    // Lambertian surfaces lit by area lights (the bench scene): the shade step, the light step and the tail compiled for that
+    // class alone (device/pb2_shade.cuh, SHADE_*).  Scenes with spheres, the lazy light distribution, image textures or the
+    // SobolSampler keep the general instantiations.
+    const bool sobol = rp.halton.sobol != nullptr;
+    const bool textured = scene->d.nTextures > 0 || sobol;
+    const bool lambertArea = scene->shadeClass == SHADE_LAMBERT_AREA && !scene->hasSpecular && !spheres;
+    const bool narrowShade = lambertArea && !scene->lazyLightDist && !textured;
     // light step: 7 resident blocks, as many as the shared-memory stage leaves room for (29 KB per block)
     AdvanceKernel advLight = spheres ? k_wf_advance<false, true, 7> : k_wf_advance<false, false, 7>;
+    if (lambertArea) advLight = k_wf_advance<false, false, 7, false, false, false, SHADE_LAMBERT_AREA>;
     AdvanceKernel advShade = scene->hasSpecular ? (spheres ? k_wf_advance<true, true, 4, true> : k_wf_advance<true, false, 4, true>)
                              : spheres ? k_wf_advance<true, true, 4>
                                        : k_wf_advance<true, false, 4>;
@@ -1075,12 +1087,12 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     // image textures: the one shade kernel that evaluates them (spheres, specular materials and the lazy light distribution
     // compiled in; 3 resident blocks, its register budget is not the bench scene's)
     // ... and the one that draws from the SobolSampler: the same general instantiation
-    const bool sobol = rp.halton.sobol != nullptr;
-    const bool textured = scene->d.nTextures > 0 || sobol;
     if (textured) advShade = k_wf_advance<true, true, 3, true, true, true>;
+    if (narrowShade) advShade = k_wf_advance<true, false, kShadeLambertAreaMinBlocks, false, false, false, SHADE_LAMBERT_AREA>;
     typedef void (*FinishKernel)(const DScene *, const DRenderParams *, WfPool, int, unsigned, float4 *);
     FinishKernel finish = scene->hasSpecular ? (spheres ? k_wf_finish<true, true> : k_wf_finish<false, true>)
                                              : (spheres ? k_wf_finish<true, false> : k_wf_finish<false, false>);
+    if (lambertArea) finish = k_wf_finish<false, false, SHADE_LAMBERT_AREA>;
     // the frame's last paths are walked to their end by one thread each once this few are left (k_wf_finish)
     static const int finishPerSM = envInt("PB2_FINISH", 256);
     // (textured scenes: the tail kernel's lane functions are the untextured instantiation, so the rounds run to the end)
@@ -1506,6 +1518,15 @@ int pb2_scene_create(const pb2_scene_desc *d, pb2_scene **out) {
     return PB2_OK;
 }
 
+static int shadeFeatureClass(const pb2_scene_desc *d);
+int pb2_shade_class(const pb2_scene_desc *d, int32_t *out) {
+    if (!d || !out) return setError(PB2_ERR_INVALID, "null argument");
+    if (d->n_materials < 0 || (d->n_materials > 0 && !d->materials) || d->n_lights < 0 || (d->n_lights > 0 && !d->lights))
+        return setError(PB2_ERR_INVALID, "bad material or light records");
+    *out = shadeFeatureClass(d);
+    return PB2_OK;
+}
+
 // ---- image textures: the MIPMap constructor (src/core/mipmap.h:112-203) on the host --------------------------------------
 // Lanczos (src/core/texture.cpp:254-262) with the default tau = 2
 static float texLanczos(float x) {
@@ -1820,6 +1841,29 @@ extern "C" int pb2_env_distribution(const pb2_texture *texture, int32_t *nu, int
     return PB2_OK;
 }
 
+// The scene's shade feature class (SHADE_* in device/pb2_shade.cuh): a bit stays clear only when no record of the scene
+// can take the branch it stands for, so the class's kernels compute what the general ones do.  PB2_SHADE_GENERAL=1 gives
+// every scene the general class (tests compare the two).
+static int shadeFeatureClass(const pb2_scene_desc *d) {
+    static const bool forceGeneral = envInt("PB2_SHADE_GENERAL", 0) != 0;
+    if (forceGeneral) return SHADE_ALL;
+    int fc = 0;
+    for (int i = 0; i < d->n_materials; ++i) {
+        const pb2_material &m = d->materials[i];
+        if (m.type == PB2_MAT_NONE) continue;
+        if (m.type == PB2_MAT_MATTE) {
+            // makeBsdf: an Oren-Nayar lobe unless clamp(sigma, 0, 90) == 0 (sigma <= 0; a NaN or textured sigma counts)
+            if (m.tex[PB2_TEX_SIGMA] || !(m.sigma <= 0.f)) fc |= SHADE_OREN_NAYAR;
+        } else if (m.type == PB2_MAT_PLASTIC)
+            fc |= SHADE_MICROFACET;
+        else
+            return SHADE_ALL;   // the specular family: the SPEC kernels, which are compiled for every class
+    }
+    for (int i = 0; i < d->n_lights; ++i)
+        if (d->lights[i].type != PB2_LIGHT_AREA) fc |= SHADE_NON_AREA;
+    return fc;
+}
+
 static int createSceneOnCurrentDevice(const pb2_scene_desc *d, pb2_scene **out) {
     int rc = PB2_OK;
     if (d->n_prims <= 0 || d->n_nodes <= 0 || !d->nodes || !d->bvh_prims || !d->prim_type || !d->prim_index)
@@ -1857,6 +1901,7 @@ static int createSceneOnCurrentDevice(const pb2_scene_desc *d, pb2_scene **out) 
         if (d->materials[i].type == PB2_MAT_MIRROR || d->materials[i].type == PB2_MAT_GLASS || d->materials[i].type == PB2_MAT_SUBSTRATE ||
             d->materials[i].type == PB2_MAT_METAL || d->materials[i].type == PB2_MAT_UBER)
             s->hasSpecular = true;
+    s->shadeClass = shadeFeatureClass(d);
     DScene &sc = s->d;
     memset(&sc, 0, sizeof(sc));
     sc.nNodes = d->n_nodes;

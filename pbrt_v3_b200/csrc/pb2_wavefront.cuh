@@ -81,10 +81,43 @@ __device__ __forceinline__ int wfLaneId() {
     return lane;
 }
 
-// Warp-collective (all 32 lanes, converged): lane l's context c (c < 0: none) is copied into warpSlots[l].  Two batches
-// of seven 16-byte loads per lane, all of a batch in flight at once.
+// Sectors of a context that a kernel reads (bit s: bytes 32 s .. 32 s + 31), staged in by wfStageIn:
+//   WF_IN_ALL    the light step: every field
+//   WF_IN_SHADE  the shade step: sectors 0-2 (state, ray, L, beta, smp, bounces, specularBounce, camRay, etaScale) and 6
+//                (hit, tHit, found, pFilm).  Sectors 3-5 (ldSum, ldLight, misTerm, misO / misD, nextO / nextD, betaNext) are
+//                dead on entry to shadeVertex: each is written by the vertex before anything reads it (lightAdvance and
+//                finishVertex read them only under the doNEE / hasMis / hasNext flags this vertex sets).  The write-back is
+//                still WF_OUT_SHADE: where the vertex does not write them, the slot's stale bytes go back to dead fields.
+enum { WF_IN_ALL = 0x7f, WF_IN_SHADE = 0x47 };
+static_assert(offsetof(DLane, etaScale) + sizeof(float) <= 96 && offsetof(DLane, smp) + sizeof(DSampler) <= 96 &&
+                  offsetof(DLane, ldSum) == 96 && offsetof(DLane, betaNext) + sizeof(V3) <= 192 && offsetof(WfCtx, hit) == 192 &&
+                  offsetof(WfCtx, pFilm) + sizeof(V2) <= 224,
+              "WF_IN_SHADE: the fields shadeVertex reads on entry lie in sectors 0-2 and 6, the dead ones in sectors 3-5");
+
+// The 16-byte chunk of a context that is the kk-th of those SECTORS cover.
+template <unsigned SECTORS>
+__device__ __forceinline__ int wfStagedChunk(int kk) {
+    if (SECTORS == WF_IN_ALL) return kk;
+    const int n = kk >> 1;
+    int s = 0, seen = 0;
+#pragma unroll
+    for (int t = 0; t < 7; ++t)
+        if ((SECTORS >> t) & 1u) {
+            s = n == seen ? t : s;
+            ++seen;
+        }
+    return 2 * s + (kk & 1);
+}
+
+// Warp-collective (all 32 lanes, converged): the SECTORS of lane l's context c (c < 0: none) are copied into
+// warpSlots[l], at their offsets.  16-byte loads in two batches per lane, all of a batch in flight at once (WF_IN_ALL:
+// seven loads each; WF_IN_SHADE: four).
+template <unsigned SECTORS = WF_IN_ALL>
 __device__ __forceinline__ void wfStageIn(const WfCtx *ctx, WfSlot *warpSlots, int c) {
-    constexpr int CHUNKS = sizeof(WfCtx) / 16, BATCH = CHUNKS / 2;
+    constexpr int NSECT = ((SECTORS >> 0) & 1) + ((SECTORS >> 1) & 1) + ((SECTORS >> 2) & 1) + ((SECTORS >> 3) & 1) +
+                          ((SECTORS >> 4) & 1) + ((SECTORS >> 5) & 1) + ((SECTORS >> 6) & 1);
+    static_assert(SECTORS <= WF_IN_ALL && NSECT > 0, "sectors of a 224-byte context");
+    constexpr int CHUNKS = 2 * NSECT, BATCH = NSECT;
     const int lane = wfLaneId();
     __syncwarp();
 #pragma unroll
@@ -93,13 +126,15 @@ __device__ __forceinline__ void wfStageIn(const WfCtx *ctx, WfSlot *warpSlots, i
         int cs[BATCH];
 #pragma unroll
         for (int it = 0; it < BATCH; ++it) {
-            const int q = (b * BATCH + it) * 32 + lane, j = q / CHUNKS, k = q % CHUNKS;
+            const int q = (b * BATCH + it) * 32 + lane, j = q / CHUNKS, kk = q % CHUNKS;
+            const int k = wfStagedChunk<SECTORS>(kk);
             cs[it] = __shfl_sync(0xffffffffu, c, j);
             if (cs[it] >= 0) v[it] = __ldcs(reinterpret_cast<const uint4 *>(ctx + cs[it]) + k);
         }
 #pragma unroll
         for (int it = 0; it < BATCH; ++it) {
-            const int q = (b * BATCH + it) * 32 + lane, j = q / CHUNKS, k = q % CHUNKS;
+            const int q = (b * BATCH + it) * 32 + lane, j = q / CHUNKS, kk = q % CHUNKS;
+            const int k = wfStagedChunk<SECTORS>(kk);
             if (cs[it] >= 0) {
                 uint2 *s = reinterpret_cast<uint2 *>(reinterpret_cast<char *>(&warpSlots[j]) + 16 * k);
                 s[0] = make_uint2(v[it].x, v[it].y);
@@ -1241,7 +1276,8 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool p
 // ---------------------------------------------------------------------------------------------
 // TEX = true: the shade step of a scene with image textures (the camera ray's differentials are rebuilt from the
 // context's pFilm); one instantiation, with everything else compiled in.
-template <bool SHADE, bool SPH, int MINB, bool SPEC = false, bool LAZY = false, bool TEX = false>
+// FC: the scene's shade feature class (SHADE_* in device/pb2_shade.cuh); SHADE_ALL is the general instantiation.
+template <bool SHADE, bool SPH, int MINB, bool SPEC = false, bool LAZY = false, bool TEX = false, int FC = SHADE_ALL>
 __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool,
                                                           int srcQ, int traceQ, int freeQ, float4 *film, unsigned long long *counters) {
     __shared__ WfSlot stage[128];
@@ -1263,7 +1299,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
         bool have = i < n;
         int c = have ? srcList[i] : 0;
         bool ended = false, deferred = false;
-        wfStageIn(pool.ctx, warpSlots, have ? c : -1);
+        wfStageIn<SHADE ? WF_IN_SHADE : WF_IN_ALL>(pool.ctx, warpSlots, have ? c : -1);
         if (have) {
             DLane &ln = slot.ln;
             const int foundCode = slot.found;
@@ -1281,8 +1317,8 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
                 tc.pFilm = slot.pFilm;
                 tc.diffScale = rp.diffScale;
                 shadeVertex<SPH, SPEC, LAZY, true>(sc, rp.halton, rp.path, ln, found, hit, tHit, u, &tc);
-            } else if (SHADE) shadeVertex<SPH, SPEC, LAZY>(sc, rp.halton, rp.path, ln, found, hit, tHit, u);
-            else lightAdvance<SPH>(sc, ln, found, hit, tHit);
+            } else if (SHADE) shadeVertex<SPH, SPEC, LAZY, false, FC>(sc, rp.halton, rp.path, ln, found, hit, tHit, u);
+            else lightAdvance<SPH, FC>(sc, ln, found, hit, tHit);
             if (SHADE && LAZY && ln.state == LS_DEFER) {
                 ln.state = LS_PATH;   // untouched: shaded again from the retry list once its voxel's record exists
                 deferred = true;
@@ -1317,7 +1353,7 @@ __device__ __forceinline__ bool wfFinishNow(const DRenderParams &rp, const WfPoo
     return n > 0 && n <= threshold && (long long)pool.ctr[CTR_WORK] >= rp.nWorkItems;
 }
 
-template <bool SPH, bool SPEC>
+template <bool SPH, bool SPEC, int FC = SHADE_ALL>
 __global__ void __launch_bounds__(128) k_wf_finish(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool, int traceQ,
                                                    unsigned threshold, float4 *film) {
     const DScene &sc = *scp;
@@ -1344,7 +1380,7 @@ __global__ void __launch_bounds__(128) k_wf_finish(const DScene *__restrict__ sc
             DHit hit;
             float tMax;
             const bool found = traceLane(sc, ln, &tMax, &hit, nullptr);
-            laneAdvance<SPH, SPEC>(sc, rp.halton, rp.path, ln, found, hit, tMax);
+            laneAdvance<SPH, SPEC, false, FC>(sc, rp.halton, rp.path, ln, found, hit, tMax);
             if (ln.state == LS_DEFER) break;            // (never: this kernel is not launched for lazily lit scenes)
             if (ln.state == LS_SHADOW) shadow++;        // the next ray is a Scene::IntersectP call
             else if (ln.state != LS_IDLE) regular++;    // ... a Scene::Intersect call
