@@ -52,6 +52,17 @@ def bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
+def nan_canonical(hits):
+    """Hit records with every NaN as 0x7fc00000: a NaN's sign and payload are not specified by IEEE 754 (x86 produces
+    0xffc00000, the device 0x7fffffff), so only NaN-ness is compared.  The reference reports hits at t = NaN for rays from
+    origins near 1e30 (the edge functions overflow); the device reports the same hits."""
+    h = hits.copy()
+    for f in h.dtype.names:
+        if h.dtype[f].base == np.float32:
+            h[f] = np.where(np.isnan(h[f]), np.float32(np.nan), h[f])
+    return h
+
+
 def row_digest(a):
     """A 32-bit digest of every bit of each row of an array of 4-byte values (FNV-1a over the words, folded): fixtures keep
     these instead of the values where the values would make them large."""
@@ -287,3 +298,345 @@ def killeroo_scene(directory, golden_dir):
         with open(path, "wb") as f:
             f.write(g[key].tobytes())
     return os.path.join(directory, KILLEROO_FILES["scene"])
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Edge scenes and rays for the trace kernels (tests/make_golden.py record_trace_edges, tests/test_gpu_trace_edges.py):
+# geometry and rays where a traversal that is only nearly the reference's gives another answer - coincident primitives
+# (the first one the reference's order reaches wins, `t < tMax` is strict), box planes shared by many nodes and flat boxes,
+# origins on box planes, rays through box corners and triangle vertices, signed zeros and infinite 1 / d, t_max at a hit's t.
+# ---------------------------------------------------------------------------------------------------------------------
+EDGE_HEADER = ('LookAt %s  %s  0 0 1\nCamera "perspective" "float fov" 45\nSampler "halton" "integer pixelsamples" 4\n'
+               'Integrator "path" "integer maxdepth" 3\nFilm "image" "integer xresolution" 32 "integer yresolution" 24\nWorldBegin\n'
+               'AttributeBegin\nAreaLightSource "diffuse" "rgb L" [6 6 6]\n'
+               'Shape "trianglemesh" "integer indices" [0 1 2 0 2 3] "point P" [%s]\nAttributeEnd\n')
+
+
+def _fmt(v):
+    return " ".join("%.9g" % x for x in np.asarray(v, np.float32).ravel())
+
+
+def _mesh(P, I, material=None):
+    m = 'Material "matte" "rgb Kd" [%s]\n' % material if material else ""
+    return m + 'Shape "trianglemesh" "integer indices" [%s] "point P" [%s]\n' % (" ".join(str(int(i)) for i in np.ravel(I)), _fmt(P))
+
+
+def _edge_header(eye, at, light_z, off=0.0):
+    lo, hi = -1 + off, 4 + off
+    light = [[lo, lo, light_z], [hi, lo, light_z], [hi, hi, light_z], [lo, hi, light_z]]
+    return EDGE_HEADER % (_fmt(eye), _fmt(at), _fmt(light))
+
+
+def _grid(n, rng, z_jitter, scale=1.0):
+    """An n x n tessellated height field over [0, 3]^2 with shared vertices: (P, I)."""
+    xs = np.linspace(0, 3, n + 1, dtype=np.float32)
+    X, Y = np.meshgrid(xs, xs)
+    Z = (1 + z_jitter * rng.uniform(-1, 1, X.shape)).astype(np.float32) * scale
+    P = np.stack([X, Y, Z], -1).reshape(-1, 3)
+    I = []
+    for j in range(n):
+        for i in range(n):
+            a = j * (n + 1) + i
+            I += [[a, a + 1, a + n + 2], [a, a + n + 2, a + n + 1]]
+    return P, np.array(I, np.int32)
+
+
+def edge_scene_text(name):
+    rng = np.random.RandomState({"coincident": 1, "coincident_wide": 2, "axis_grid": 3, "axis_grid_far": 3, "fan": 4, "spheres": 5,
+                                 "instances": 6}[name])
+    floor = _mesh([[-2, -2, 0], [5, -2, 0], [5, 5, 0], [-2, 5, 0]], [[0, 1, 2], [0, 2, 3]], ".5 .5 .5")
+    if name in ("coincident", "coincident_wide"):
+        # a mesh, then copies of it: identical with another material, reversed winding, vertex order rotated
+        P, I = _grid(8 if name == "coincident" else 4, rng, 0.2)
+        text = _edge_header((1.5, -4, 4), (1.5, 1.5, 1), 4) + floor + _mesh(P, I, ".7 .2 .2") + _mesh(P, I, ".2 .7 .2")
+        text += _mesh(P, I[:, ::-1], ".2 .2 .7") + _mesh(P, I[:, [1, 2, 0]], ".7 .7 .2")
+        if name == "coincident_wide":
+            # 18 more copies of three triangles: their centroid bounds are degenerate, so each ends in a leaf of 22 (> 16)
+            for k in range(18):
+                text += _mesh(P, I[[0, 7, 20]][:, [[0, 1, 2], [1, 2, 0], [2, 0, 1]][k % 3]], "%.2f .5 .5" % (0.1 + 0.04 * k))
+        return text + "WorldEnd\n"
+    if name in ("axis_grid", "axis_grid_far"):
+        # unit cubes and axis-aligned quads on an integer lattice: node boxes share planes, quads make flat boxes
+        off = 1e5 if name == "axis_grid_far" else 0.0
+        cube_P = np.array([[0, 0, 0], [1, 0, 0], [1, 1, 0], [0, 1, 0], [0, 0, 1], [1, 0, 1], [1, 1, 1], [0, 1, 1]], np.float32)
+        cube_I = np.array([[0, 2, 1], [0, 3, 2], [4, 5, 6], [4, 6, 7], [0, 1, 5], [0, 5, 4], [1, 2, 6], [1, 6, 5], [2, 3, 7], [2, 7, 6],
+                           [3, 0, 4], [3, 4, 7]], np.int32)
+        quad_I = np.array([[0, 1, 2], [0, 2, 3]], np.int32)
+        text = _edge_header((1.5 + off, -5 + off, 5), (1.5 + off, 1.5 + off, 1), 5, off)
+        text += _mesh(np.float32([[-2, -2, 0], [5, -2, 0], [5, 5, 0], [-2, 5, 0]]) + np.float32([off, off, 0]), quad_I, ".5 .5 .5")
+        cells = [(x, y, z) for x in range(4) for y in range(4) for z in range(3)]
+        for k in rng.permutation(len(cells))[:22]:
+            x, y, z = cells[k]
+            text += _mesh(cube_P + np.float32([x + off, y + off, z]), cube_I, "%.2f .4 .6" % (0.2 + 0.02 * x))
+        for k in range(24):
+            axis, c = rng.randint(3), rng.randint(0, 4)
+            a0, b0 = rng.randint(0, 3, 2)
+            sa, sb = rng.randint(1, 3, 2)
+            q = np.zeros((4, 3), np.float32)
+            u, v = (axis + 1) % 3, (axis + 2) % 3
+            q[:, axis] = c
+            q[:, u] = [a0, a0 + sa, a0 + sa, a0]
+            q[:, v] = [b0, b0, b0 + sb, b0 + sb]
+            text += _mesh(q + np.float32([off, off, 0]), quad_I, ".6 .6 %.2f" % (0.1 + 0.03 * k))
+        return text + "WorldEnd\n"
+    if name == "fan":
+        # a tessellated grid and triangle fans: many triangles share a vertex, rays go through shared vertices and edges
+        P, I = _grid(12, rng, 0.0)
+        text = _edge_header((1.5, -4, 4), (1.5, 1.5, 1), 4) + floor + _mesh(P, I, ".6 .3 .3")
+        for k in range(6):
+            c = np.float32([rng.uniform(0, 3), rng.uniform(0, 3), rng.uniform(1.5, 2.5)])
+            m = 8 + 4 * k
+            ang = np.linspace(0, 2 * np.pi, m, endpoint=False)
+            r = rng.uniform(0.3, 0.7)
+            ring = np.stack([c[0] + r * np.cos(ang), c[1] + r * np.sin(ang), c[2] + 0.2 * np.sin(3 * ang)], 1)
+            FP = np.concatenate([c[None], ring]).astype(np.float32)
+            FI = [[0, 1 + i, 1 + (i + 1) % m] for i in range(m)]
+            text += _mesh(FP, FI, ".3 .6 .%d" % k)
+        return text + "WorldEnd\n"
+    if name == "spheres":
+        text = _edge_header((1.5, -5, 4), (1.5, 1.5, 1), 5) + floor
+        shapes = [(0.5, 0.5, 1, 'Shape "sphere" "float radius" .8'),
+                  (2.5, 0.5, 1, 'Shape "sphere" "float radius" .8 "float phimax" 270'),
+                  (0.5, 2.5, 1, 'Shape "sphere" "float radius" .8 "float zmin" -.5 "float zmax" .6'),
+                  (2.5, 2.5, 1, 'Shape "sphere" "float radius" .8 "float zmin" -.7 "float zmax" .3 "float phimax" 200'),
+                  (1.5, 1.5, 2, 'Shape "sphere" "float radius" .6'),
+                  (1.5, 1.5, 2, 'Shape "sphere" "float radius" .6')]   # two coincident spheres
+        for k, (x, y, z, s) in enumerate(shapes):
+            text += 'AttributeBegin\nTranslate %g %g %g\nMaterial "matte" "rgb Kd" [.%d .5 .5]\n%s\nAttributeEnd\n' % (x, y, z, k + 1, s)
+        return text + "WorldEnd\n"
+    if name == "instances":
+        P, I = _grid(3, rng, 0.3, 0.5)
+        text = _edge_header((1.5, -5, 4), (1.5, 1.5, 1), 5) + floor
+        text += 'ObjectBegin "patch"\n' + _mesh(P * np.float32(0.5), I, ".6 .4 .2") + 'Shape "sphere" "float radius" .2\nObjectEnd\n'
+        for tr in ("Translate 0 0 .5", "Translate 0 0 .5", "Translate 3 0 .5\nScale -1 1 1", "Translate 1 1.5 1\nRotate 30 0 0 1"):
+            text += "AttributeBegin\n%s\nObjectInstance \"patch\"\nAttributeEnd\n" % tr
+        return text + "WorldEnd\n"
+    raise KeyError(name)
+
+
+# name -> maxnodeprims of the SAH build
+EDGE_SCENES = {"coincident": 4, "coincident_wide": 4, "axis_grid": 4, "axis_grid_far": 4, "fan": 4, "spheres": 4, "instances": 4}
+SHADOW_EPSILON = np.float32(0.0001)
+SLAB_SCALE = np.float32(1) + np.float32(2) * ((np.float32(3) * np.float32(2.0 ** -24)) / (np.float32(1) - np.float32(3) * np.float32(2.0 ** -24)))
+
+
+def edge_scene(pb, name):
+    return pb.HostScene.from_string(with_accelerator(edge_scene_text(name), "sah", EDGE_SCENES[name]))
+
+
+def slab_events(o, d, bmin, bmax, t_max):
+    """Bounds3::IntersectP (geometry.h:1412-1438) in float32 without FMA for rays (n, 3) against boxes (m, 3), (n, m) each:
+    the verdict, and whether the test met an exact equality - an entry parameter equal to the exit parameter it is compared
+    with, or the origin on one of the box's planes (slab value 0 * inf = NaN for axis-parallel rays)."""
+    f = np.float32
+    with np.errstate(all="ignore"):
+        inv = (f(1) / d.astype(f))[:, None, :]
+        neg = inv < 0
+        o = o.astype(f)[:, None, :]
+        near = np.where(neg, bmax[None], bmin[None]).astype(f)
+        far = np.where(neg, bmin[None], bmax[None]).astype(f)
+        dn, df = (near - o).astype(f), (far - o).astype(f)
+        t0 = (dn * inv).astype(f)
+        t1 = ((df * inv).astype(f) * SLAB_SCALE).astype(f)
+        on_plane = ((dn == 0) | (df == 0)).any(-1)
+        tmin, tmax = t0[..., 0], t1[..., 0]
+        eq = (tmin == t1[..., 1]) | (t0[..., 1] == tmax)
+        ok = ~((tmin > t1[..., 1]) | (t0[..., 1] > tmax))
+        tmin = np.where(t0[..., 1] > tmin, t0[..., 1], tmin)
+        tmax = np.where(t1[..., 1] < tmax, t1[..., 1], tmax)
+        eq |= (tmin == t1[..., 2]) | (t0[..., 2] == tmax)
+        ok &= ~((tmin > t1[..., 2]) | (t0[..., 2] > tmax))
+        tmin = np.where(t0[..., 2] > tmin, t0[..., 2], tmin)
+        tmax = np.where(t1[..., 2] < tmax, t1[..., 2], tmax)
+        ok &= (tmin < np.asarray(t_max, f)[:, None]) & (tmax > 0)
+    return ok, eq | on_plane
+
+
+def reached_box_equalities(nodes, rays, t_final):
+    """Per ray: some box test of the reference's traversal met an exact equality (slab_events).  The boxes counted are the
+    root's and those of children of nodes the ray passes with its final tMax: every one of them the reference tests."""
+    ok, eq = slab_events(rays["o"], rays["d"], nodes["bmin"], nodes["bmax"], t_final)
+    parent = np.full(len(nodes), -1)
+    interior = np.flatnonzero(nodes["n_prims"] == 0)
+    parent[interior + 1] = interior
+    parent[nodes["offset"][interior]] = interior
+    reached = np.ones_like(ok)
+    reached[:, 1:] = ok[:, parent[1:]]
+    return (eq & reached).any(1)
+
+
+def slow_rays(rays):
+    """Rays whose origin or 1 / d is not finite: the kernels test their boxes with the reference's exact sequence."""
+    with np.errstate(divide="ignore", over="ignore"):
+        return ~(np.isfinite(np.float32(1) / rays["d"]).all(1) & np.isfinite(rays["o"]).all(1))
+
+
+def _unit(v):
+    return (v / np.linalg.norm(v, axis=-1, keepdims=True)).astype(np.float32)
+
+
+def edge_rays(pb, hs, closest, n_per_family=200, seed=0):
+    """Path rays and shadow rays of the edge families for a scene (closest: Scene::Intersect of the reference, for the
+    t_max family and the shadow segments).  Returns (rays, shadow rays, family of each ray)."""
+    rng = np.random.RandomState(seed)
+    f = np.float32
+    nodes = hs.nodes()
+    lo, hi = nodes["bmin"][0], nodes["bmax"][0]
+    ext = (hi - lo).astype(f)
+    d = hs.desc.contents
+    tri_type = np.ctypeslib.as_array(d.prim_type, shape=(d.n_prims,))
+    P = np.ctypeslib.as_array(d.P, shape=(d.n_vertices, 3)).copy() if d.n_vertices else np.zeros((0, 3), f)
+    TI = np.ctypeslib.as_array(d.tri_index, shape=(d.n_tris, 3)).copy() if d.n_tris else np.zeros((0, 3), np.int32)
+    n = n_per_family
+
+    def inside(k, margin=0.1):
+        return rng.uniform(lo - margin * ext, hi + margin * ext, (k, 3)).astype(f)
+
+    def aim(o, target):
+        with np.errstate(all="ignore"):
+            return (target.astype(f) - o.astype(f)).astype(f)
+
+    fams = []
+    # 1. origins with one or two coordinates exactly on a node's bmin / bmax plane
+    k = rng.randint(0, len(nodes), n)
+    o = inside(n)
+    for j in range(n):
+        for ax in rng.choice(3, 1 + (j % 2), replace=False):
+            o[j, ax] = (nodes["bmin"] if rng.rand() < .5 else nodes["bmax"])[k[j], ax]
+    dd = _unit(rng.normal(size=(n, 3)))
+    half = n // 2
+    dd[:half] = aim(o[:half], inside(half, 0.0))
+    fams.append(("box_planes", o, dd))
+    # 2. +0 / -0 components, exactly axis-parallel, 1e-30 components (finite 1 / d, overflowing products), denormals
+    o = inside(n)
+    dd = _unit(aim(o, inside(n, 0.0)))
+    kind = np.arange(n) % 6
+    for j in range(n):
+        ax = rng.randint(3)
+        if kind[j] == 0:
+            dd[j, ax] = f(0.0)
+        elif kind[j] == 1:
+            dd[j, ax] = f(-0.0)
+        elif kind[j] == 2:
+            s = f(1.0) if rng.rand() < .5 else f(-1.0)
+            dd[j] = f(-0.0) if rng.rand() < .5 else f(0.0)
+            dd[j, ax] = s
+        elif kind[j] == 3:
+            dd[j, ax] = f(1e-30) * (1 if rng.rand() < .5 else -1)
+        elif kind[j] == 4:
+            dd[j, ax] = f(1e-40) * (1 if rng.rand() < .5 else -1)
+    fams.append(("directions", o, dd))
+    # 3. aimed at node-box corners and edge points, nudged by ulps until an entry parameter EQUALS an exit parameter
+    k = rng.randint(0, len(nodes), n)
+    corner_sel = rng.randint(0, 2, (n, 3))
+    tgt = np.where(corner_sel == 0, nodes["bmin"][k], nodes["bmax"][k]).astype(f)
+    edge = np.arange(n) % 2 == 1
+    ax = rng.randint(0, 3, n)
+    mid = ((nodes["bmin"][k] + nodes["bmax"][k]) * f(0.5)).astype(f)
+    tgt[edge, ax[edge]] = mid[edge, ax[edge]]
+    o = (tgt + _unit(rng.normal(size=(n, 3))) * ext.max() * f(0.6)).astype(f)
+    dd = aim(o, tgt)
+    best = dd.copy()
+    for j in range(n):
+        bmin, bmax = nodes["bmin"][k[j]][None], nodes["bmax"][k[j]][None]
+        cand = np.repeat(dd[j][None], 3 * 33, 0)
+        steps = np.tile(np.arange(-16, 17), 3)
+        axes = np.repeat(np.arange(3), 33)
+        vals = cand[np.arange(len(cand)), axes]
+        for s in range(len(cand)):
+            v = vals[s]
+            for _ in range(abs(steps[s])):
+                v = np.nextafter(v, f(np.inf) if steps[s] > 0 else f(-np.inf))
+            cand[s, axes[s]] = v
+        ok, eq = slab_events(np.repeat(o[j][None], len(cand), 0), cand, bmin, bmax, np.full(len(cand), np.inf, f))
+        hitq = np.flatnonzero(eq[:, 0] & ok[:, 0])
+        if len(hitq):
+            best[j] = cand[hitq[np.argmin(np.abs(steps[hitq]))]]
+    fams.append(("corners", o, best))
+    # 4. aimed at triangle vertices and at float midpoints of triangle edges
+    if len(TI):
+        t = rng.randint(0, len(TI), n)
+        v = rng.randint(0, 3, n)
+        tgt = P[TI[t, v]].astype(f)
+        m = np.arange(n) % 2 == 1
+        tgt[m] = ((P[TI[t, v]][m] + P[TI[t, (v + 1) % 3]][m]) * f(0.5)).astype(f)
+        o = (tgt + _unit(rng.normal(size=(n, 3))) * ext.max() * f(0.5)).astype(f)
+        fams.append(("vertices", o, aim(o, tgt)))
+    # 5. t_max at a reference hit's t, one ulp either side of it, +0, -0, negative
+    o = inside(n, 0.0)
+    dd = _unit(aim(o, inside(n, 0.0)))
+    fams.append(("tmax", o, dd))
+    # 6. non-finite origins, and far origins (|o| ~ 1e30) aimed at the scene
+    o = inside(n)
+    dd = _unit(aim(o, inside(n, 0.0)))
+    m = np.arange(n) % 2 == 0
+    o[m, rng.randint(0, 3, m.sum())] = np.where(rng.rand(m.sum()) < .5, f(np.inf), f(-np.inf))
+    far = ~m
+    w = _unit(rng.normal(size=(far.sum(), 3)))
+    c = ((lo + hi) * f(0.5)).astype(f)
+    o[far] = (c + w * f(1e30)).astype(f)
+    dd[far] = -w
+    fams.append(("nonfinite", o, dd))
+
+    names = [nm for nm, _, _ in fams]
+    fam = np.concatenate([np.full(len(a), i, np.int32) for i, (_, a, _) in enumerate(fams)])
+    rays = np.zeros(len(fam), pb.RAY_DTYPE)
+    rays["o"] = np.concatenate([a for _, a, _ in fams])
+    rays["d"] = np.concatenate([b for _, _, b in fams])
+    rays["t_max"] = np.inf
+    tm = fam == names.index("tmax")
+    h = closest(rays)
+    t = h["t"][tm]
+    choice = np.arange(tm.sum()) % 6
+    with np.errstate(all="ignore"):
+        tmax = np.select([choice == 0, choice == 1, choice == 2, choice == 3, choice == 4],
+                         [t, np.nextafter(t, f(np.inf)), np.nextafter(t, f(-np.inf)), f(0.0), f(-0.0)], f(-1.0)).astype(f)
+    tmax[(h["prim"][tm] < 0) & (choice < 3)] = np.inf
+    rays["t_max"][tm] = tmax
+    h = closest(rays)
+    # shadow rays: the same origins, segments that end exactly at the reference's hit point (or far beyond a miss)
+    srays = rays.copy()
+    srays["t_max"] = f(1) - SHADOW_EPSILON
+    hit = h["prim"] >= 0
+    with np.errstate(all="ignore"):
+        srays["d"][hit] = (h["p"][hit] - rays["o"][hit]).astype(f)
+        srays["d"][~hit] = (rays["d"][~hit] * ext.max() * f(2)).astype(f)
+    return rays, srays, fam, names
+
+
+def coincident_prims(hs):
+    """Per scene primitive: another primitive covers exactly the same triangle (same three vertex positions in any order)
+    or is the same sphere."""
+    d = hs.desc.contents
+    ptype = np.ctypeslib.as_array(d.prim_type, shape=(d.n_prims,))
+    pidx = np.ctypeslib.as_array(d.prim_index, shape=(d.n_prims,))
+    out = np.zeros(d.n_prims, bool)
+    keys = {}
+    P = np.ctypeslib.as_array(d.P, shape=(d.n_vertices, 3)) if d.n_vertices else None
+    TI = np.ctypeslib.as_array(d.tri_index, shape=(d.n_tris, 3)) if d.n_tris else None
+    for i in range(d.n_prims):
+        if ptype[i] == 0:
+            key = (0,) + tuple(sorted(P[TI[pidx[i]]].astype(np.float32).tobytes()[12 * j:12 * j + 12] for j in range(3)))
+        elif ptype[i] == 1:
+            s = d.spheres[pidx[i]]
+            key = (1, bytes(s))
+        else:
+            continue
+        keys.setdefault(key, []).append(i)
+    for v in keys.values():
+        if len(v) > 1:
+            out[v] = True
+    return out
+
+
+def edge_coverage(hs, nodes, rays, hits):
+    """What the edge rays of a scene reach (floors on these keep the fixture from being weakened quietly)."""
+    prim = hits["prim"]
+    coinc = coincident_prims(hs)
+    on_coincident = (prim >= 0) & coinc[np.clip(prim, 0, len(coinc) - 1)]
+    t_final = np.where(prim >= 0, hits["t"], rays["t_max"]).astype(np.float32)
+    return {"coincident_hits": int(on_coincident.sum()),
+            "box_equalities": int(reached_box_equalities(nodes, rays, t_final).sum()),
+            "negative_zero": int((np.signbit(rays["d"]) & (rays["d"] == 0)).any(1).sum()),
+            "slow": int(slow_rays(rays).sum()),
+            "hits": int((prim >= 0).sum())}

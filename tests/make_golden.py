@@ -4,6 +4,9 @@ Run where the reference's source tree is, after __graft_entry__.build():
 
     PBRT_V3_DIR=<the reference's source tree> python tests/make_golden.py
 
+`python tests/make_golden.py trace_edges` records tests/golden/trace_edges.npz alone and adds the exact-parity
+fixture's "coincident" case to it.
+
 The fixtures travel with the repo; the tests compare the oracle port (everywhere) and the CUDA path (on a GPU)
 against them, so that parity is pinned to the reference where it does not exist.
 """
@@ -169,6 +172,31 @@ def record_sobol_tables(ref):
     print("sobol tables", mats.shape, tabs.shape)
 
 
+def record_trace_edges(ref):
+    """For every edge scene of tests/golden_cases.py (EDGE_SCENES), with the reference in device-math mode (a partial
+    sphere's phi goes through atan2): its canonical LinearBVHNode array and primitive order, the edge rays and shadow rays, Scene::Intersect of
+    the rays (prim and t raw, every field but the barycentrics, which the reference does not expose, as a row digest of the
+    record with NaNs made canonical) and
+    Scene::IntersectP of the shadow rays."""
+    import test_gpu_exact_parity
+    out = {}
+    with ref.device_math():
+        for name, mp in gc.EDGE_SCENES.items():
+            hs = gc.edge_scene(pb, name)
+            sc = ref.scene(hs, max_prims_in_node=mp)
+            rays, srays, fam, fam_names = gc.edge_rays(pb, hs, sc.intersect)
+            hits = sc.intersect(rays)
+            nodes, prims = sc.bvh()
+            out[name + ":nodes"], out[name + ":prims"] = canonical_nodes(nodes), prims
+            out[name + ":rays"], out[name + ":srays"], out[name + ":family"] = rays, srays, fam
+            out[name + ":prim"], out[name + ":t"] = hits["prim"], hits["t"]
+            out[name + ":digest"] = gc.row_digest(test_gpu_exact_parity.hit_rows(gc.nan_canonical(hits)))
+            out[name + ":occluded"] = sc.intersect_p(srays)
+            print("trace edges", name, len(nodes), "nodes", gc.edge_coverage(hs, hs.nodes(), rays, hits))
+    out["families"] = np.array(fam_names)
+    np.savez_compressed(os.path.join(OUT, "trace_edges.npz"), **out)
+
+
 def record_killeroo_scene(ref_dir):
     """The reference's scenes/killeroo-simple.pbrt and the geometry it includes, stored as bytes (scene data, no source)."""
     scenes = os.path.join(ref_dir, "scenes")
@@ -220,6 +248,15 @@ def record_openexr_images(ref_dir):
 
 
 def main():
+    if sys.argv[1:] == ["trace_edges"]:
+        # the edge-ray fixture alone, and the exact-parity fixture's coincident case added to its other (unchanged) entries
+        ref = pyoracle.reference()
+        if ref is None:
+            raise SystemExit("oracle/_ref is not built: run `make -C oracle -f Makefile.ref REF=$PBRT_V3_DIR`")
+        record_trace_edges(ref)
+        import test_gpu_exact_parity
+        test_gpu_exact_parity.record_reference(ref, os.path.join(OUT, "exact_parity.npz"), only=["coincident"])
+        return
     ref_dir = os.environ.get("PBRT_V3_DIR")
     if not ref_dir or not os.path.isdir(os.path.join(ref_dir, "src")):
         raise SystemExit("set PBRT_V3_DIR to the reference's source tree (the directory that holds src/ and scenes/)")
@@ -259,6 +296,7 @@ def main():
     record_openexr_images(ref_dir)
     record_filters(ref)
     record_hlbvh(ref)
+    record_trace_edges(ref)
     # the reference in device-math mode, for tests/test_gpu_exact_parity.py
     import test_gpu_exact_parity
     test_gpu_exact_parity.record_reference(ref, os.path.join(OUT, "exact_parity.npz"))

@@ -43,7 +43,7 @@ TESTS = os.path.dirname(os.path.abspath(__file__))
 EXCEPTIONS = {}
 
 EXTRA_CASES = ["analytic_" + c for c in sorted(gc.ANALYTIC_SCENES)] + ["filter_" + c for c in sorted(gc.FILTER_CASES)] + \
-              ["soup20k", "instanced_soup", "emissive_mesh", "lights_spatial", "lights_uniform", "one_sided_lights"]
+              ["soup20k", "instanced_soup", "emissive_mesh", "lights_spatial", "lights_uniform", "one_sided_lights", "coincident"]
 CASES = SCENE_CASES + EXTRA_CASES
 MODELLED_FILTERS = ("box", "gaussian")    # film_model's filter tables
 
@@ -65,6 +65,8 @@ def make_case(pb, case):
         return pb.HostScene.from_string(gc.lights_text(SCENES, case.split("_")[1]))
     if case == "one_sided_lights":
         return pb.HostScene.from_string(ONE_SIDED_LIGHTS)
+    if case == "coincident":   # coincident triangles of four materials: the tied primitive the traversal reports picks the material
+        return gc.edge_scene(pb, case)
     raise KeyError(case)
 
 
@@ -100,13 +102,14 @@ def hit_rows(hits):
     return h
 
 
-def record_reference(ref, path):
+def record_reference(ref, path, only=None):
     """What the compiled reference computes in device-math mode for every check of this file (run by tests/make_golden.py):
-    per-pixel digests of every work item's L and pFilm, ray counters, hit / light-distribution / look-up digests."""
+    per-pixel digests of every work item's L and pFilm, ray counters, hit / light-distribution / look-up digests.
+    only: record just these cases and add them to the existing fixture, whose other entries are kept as they are."""
     import pbrt_v3_b200 as pb
     out = {}
     with ref.device_math():
-        for case in CASES:
+        for case in only or CASES:
             hs = make_case(pb, case)
             _, pix, sn = frame_items(hs)
             sc = ref.scene(hs)
@@ -119,6 +122,11 @@ def record_reference(ref, path):
                 out[case + ":occluded"] = sc.intersect_p(gc.rays_for(pb, nodes, 1500, 12, shadow=True))
                 out[case + ":light_distribution"] = gc.row_digest(sc.light_distribution(gc.points_for(nodes, 400, 15)))
             del sc
+        if only:
+            old = np.load(path)
+            assert not set(out) & set(old.files), "only adds cases that are not in the fixture yet"
+            np.savez_compressed(path, **{k: old[k] for k in old.files}, **out)
+            return
         for i, t in enumerate(make_case(pb, "textured").textures()):
             st, dst = gc.texture_lookup_inputs(3000, 100 + i)
             out["lookup_%d" % i] = gc.row_digest(ref.texture_lookup(t, st, dst))

@@ -842,3 +842,15 @@ def test_openexr_reader(pb, tmp_path):
     with pytest.raises(RuntimeError):
         pb.read_image(os.path.join(ilm, "comp_b44.exr"))
     assert pb.lib().pb2h_error_count() > before
+
+
+@pytest.mark.parametrize("name", list(gc.EDGE_SCENES))
+def test_host_bvh_equals_reference_bvh_on_edge_scenes(pb, name):
+    """Coincident copies of a mesh (equal centroids, and leaves of more than 16 primitives where the centroid bounds are
+    degenerate), lattice cubes and quads, fans, coincident spheres, instances: the host SAH builder orders ties of equal
+    centroids (nth_element / partition) as BVHAccel does - node array and primitive order equal the reference's
+    (tests/golden/trace_edges.npz)."""
+    g = np.load(os.path.join(GOLDEN, "trace_edges.npz"))
+    hs = gc.edge_scene(pb, name)
+    assert same_bvh(hs.nodes(), g[name + ":nodes"])
+    assert np.array_equal(hs.bvh_prims(), g[name + ":prims"])

@@ -463,3 +463,56 @@ def test_shade_kernel_bsdf_functions_match_the_reference_bsdf(pb, scene):
         assert (want[:, 17] != 0).mean() > 0.3   # (half of the frames see the surface from below the shading hemisphere or so)
         types.add(d.materials[m].type)
     assert pb.PB2_MAT_MATTE in types
+
+
+EDGE_FLOORS = dict(box_equalities=120, negative_zero=40, slow=200, hits=400)
+
+
+@pytest.mark.parametrize("name", list(gc.EDGE_SCENES))
+def test_port_matches_reference_on_edge_rays(pb, port, name):
+    """The edge rays (tests/golden_cases.py edge_rays: origins on box planes, +-0 / 1e-30 / denormal direction components,
+    rays aimed at box corners and triangle vertices, t_max at a hit's t and one ulp either side, non-finite and far
+    origins) through Scene::Intersect / IntersectP of the port: prim, t and every other hit field BIT FOR BIT what the
+    reference recorded (tests/golden/trace_edges.npz), and live against the compiled reference where it was built.  The
+    recording ran with the device's transcendentals, the port calls glibc's: a sphere hit's n, dpdu and uv (acos, atan2) are
+    compared live only."""
+    from oracle import pyoracle
+    from test_gpu_exact_parity import hit_rows
+    g = np.load(os.path.join(GOLDEN, "trace_edges.npz"))
+    hs = gc.edge_scene(pb, name)
+    sc = port.scene(hs, max_prims_in_node=gc.EDGE_SCENES[name])
+    rays, srays = g[name + ":rays"], g[name + ":srays"]
+    hits = sc.intersect(rays)
+    assert np.array_equal(hits["prim"], g[name + ":prim"])
+    assert np.array_equal(gc.bits(hits["t"]), gc.bits(g[name + ":t"]))
+    d = hs.desc.contents
+    prim_type = np.ctypeslib.as_array(d.prim_type, shape=(d.n_prims,))
+    sphere = (hits["prim"] >= 0) & (prim_type[np.maximum(hits["prim"], 0)] == pb.PB2_PRIM_SPHERE)
+    bad = np.flatnonzero((gc.row_digest(hit_rows(gc.nan_canonical(hits))) != g[name + ":digest"]) & ~sphere)
+    assert len(bad) == 0, "hit fields differ for rays %s" % bad[:10].tolist()
+    assert np.array_equal(sc.intersect_p(srays), g[name + ":occluded"])
+    ref = pyoracle.reference()
+    if ref is not None:
+        rs = ref.scene(hs, max_prims_in_node=gc.EDGE_SCENES[name])
+        assert hits.tobytes() == rs.intersect(rays).tobytes()
+        assert np.array_equal(sc.intersect_p(srays), rs.intersect_p(srays))
+
+
+@pytest.mark.parametrize("name", list(gc.EDGE_SCENES))
+def test_edge_rays_reach_the_edges(pb, port, name):
+    """The generator reproduces the recorded rays, and they reach what they are there for: per scene, rays for which a box
+    test of the reference's traversal meets an exact equality (entry parameter equal to an exit parameter, or the origin on
+    a box plane; Bounds3::IntersectP emulated in float32), rays with a -0 direction component, rays the kernels must test
+    with the exact compare sequence (non-finite origin or 1 / d), hits; and hits on coincident geometry."""
+    g = np.load(os.path.join(GOLDEN, "trace_edges.npz"))
+    hs = gc.edge_scene(pb, name)
+    sc = port.scene(hs, max_prims_in_node=gc.EDGE_SCENES[name])
+    rays, srays, fam, names = gc.edge_rays(pb, hs, sc.intersect)
+    assert rays.tobytes() == g[name + ":rays"].tobytes() and srays.tobytes() == g[name + ":srays"].tobytes()
+    assert np.array_equal(fam, g[name + ":family"]) and list(names) == list(g["families"])
+    cov = gc.edge_coverage(hs, hs.nodes(), rays, sc.intersect(rays))
+    for key, floor in EDGE_FLOORS.items():
+        assert cov[key] >= floor, (key, cov)
+    assert cov["coincident_hits"] >= {"coincident": 200, "coincident_wide": 200, "axis_grid": 20, "axis_grid_far": 20, "spheres": 15}.get(name, 0), cov
+    if name == "coincident_wide":
+        assert hs.nodes()["n_prims"].max() > 16   # beyond the two-child records: the 32-B-node kernel traces this scene
