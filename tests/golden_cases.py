@@ -112,6 +112,15 @@ def filter_scene_text(scene_dir, case):
     return text.replace("WorldBegin", pixel_filter + "\nWorldBegin", 1)
 
 
+def scene_file_text(scene_dir, name):
+    """tests/scenes/<name>.pbrt as one text that parses from anywhere: its Includes inlined, the files it reads (textures/)
+    named by absolute path."""
+    import re
+    text = open(os.path.join(scene_dir, name + ".pbrt")).read()
+    text = re.sub(r'Include "([^"]+)"', lambda m: open(os.path.join(scene_dir, m.group(1))).read(), text)
+    return text.replace('"textures/', '"%s/' % os.path.join(scene_dir, "textures"))
+
+
 def with_accelerator(text, split, maxprims, device_build=False):
     extra = ' "bool devicebuild" "true"' if device_build else ""
     return text.replace("WorldBegin", 'Accelerator "bvh" "string splitmethod" "%s" "integer maxnodeprims" [%d]%s\nWorldBegin' % (split, maxprims, extra), 1)

@@ -5,7 +5,7 @@ Run where the reference's source tree is, after __graft_entry__.build():
     PBRT_V3_DIR=<the reference's source tree> python tests/make_golden.py
 
 `python tests/make_golden.py trace_edges` records tests/golden/trace_edges.npz alone and adds the exact-parity
-fixture's "coincident" case to it.
+fixture's "coincident" case to it.  `python tests/make_golden.py one_sample` records tests/golden/one_sample.npz alone.
 
 The fixtures travel with the repo; the tests compare the oracle port (everywhere) and the CUDA path (on a GPU)
 against them, so that parity is pinned to the reference where it does not exist.
@@ -257,6 +257,13 @@ def main():
         import test_gpu_exact_parity
         test_gpu_exact_parity.record_reference(ref, os.path.join(OUT, "exact_parity.npz"), only=["coincident"])
         return
+    if sys.argv[1:] == ["one_sample"]:
+        ref = pyoracle.reference()
+        if ref is None:
+            raise SystemExit("oracle/_ref is not built: run `make -C oracle -f Makefile.ref REF=$PBRT_V3_DIR`")
+        import test_gpu_sample_films
+        test_gpu_sample_films.record_reference(ref, os.path.join(OUT, "one_sample.npz"))
+        return
     ref_dir = os.environ.get("PBRT_V3_DIR")
     if not ref_dir or not os.path.isdir(os.path.join(ref_dir, "src")):
         raise SystemExit("set PBRT_V3_DIR to the reference's source tree (the directory that holds src/ and scenes/)")
@@ -301,6 +308,10 @@ def main():
     import test_gpu_exact_parity
     test_gpu_exact_parity.record_reference(ref, os.path.join(OUT, "exact_parity.npz"))
     print("exact parity fixture written")
+    # ... and of the one-sample frames, for tests/test_gpu_sample_films.py
+    import test_gpu_sample_films
+    test_gpu_sample_films.record_reference(ref, os.path.join(OUT, "one_sample.npz"))
+    print("one-sample fixture written")
     # the metal material's default eta / k: copper's measured spectra through Spectrum::FromSampled (metal.cpp:121-126)
     eta, k = ref.copper_rgb()
     np.savez_compressed(os.path.join(OUT, "metal_defaults.npz"), eta=eta, k=k)

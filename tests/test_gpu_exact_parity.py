@@ -12,8 +12,9 @@ into tests/golden/exact_parity.npz as 32-bit digests of every bit (the values th
   * golden scenes: pb2_intersect's every field (spheres' n, ns, dpdu, uv included; not the barycentrics, which the
     reference does not expose), pb2_intersect_p, the light distributions and the textured scene's MIPMap look-ups;
   * films of the benchmarked kernels, with the shipped settings and with every bounce through the round kernels
-    (PB2_FINISH=0), against the float64 film model of the samples (test_gpu_wavefront_schedules.film_model), which the first
-    check makes the reference's: weight channel of box-filtered films exact, every RGB value within k * 2^-24 * sum |L w|;
+    (PB2_FINISH=0), against the float64 film model of the samples (test_gpu_wavefront_schedules.film_model, every filter),
+    which the first check makes the reference's: weight channel of box-filtered films exact, every RGB value within
+    k * 2^-24 * sum |L w|;
   * camera, regular and shadow ray counters equal to the reference's SamplerIntegrator::Render;
   * the full-size benchmark scene on 32 x 32 blocks of five crop windows.
 
@@ -45,7 +46,7 @@ EXCEPTIONS = {}
 EXTRA_CASES = ["analytic_" + c for c in sorted(gc.ANALYTIC_SCENES)] + ["filter_" + c for c in sorted(gc.FILTER_CASES)] + \
               ["soup20k", "instanced_soup", "emissive_mesh", "lights_spatial", "lights_uniform", "one_sided_lights", "coincident"]
 CASES = SCENE_CASES + EXTRA_CASES
-MODELLED_FILTERS = ("box", "gaussian")    # film_model's filter tables
+MODELLED_FILTERS = ("box", "gaussian", "mitchell", "sinc", "triangle")    # film_model's filter tables
 
 
 def make_case(pb, case):
@@ -215,10 +216,11 @@ def test_every_sample_film_and_counter_equals_the_reference(pb, want, rounds, ca
     assert counters(st) == ref_rays, "shipped settings: ray counters"
     assert tuple(int(v) for v in rounds[case + ":stats"]) == ref_rays, "PB2_FINISH=0: ray counters"
     film = hs.film.contents
-    kind = {pb.PB2_FILTER_BOX: "box", pb.PB2_FILTER_GAUSSIAN: "gaussian"}.get(film.filter_type)
-    if kind not in MODELLED_FILTERS:
-        return    # mitchell / sinc / triangle: the samples and the counters above are what this file checks
-    # the samples equal the reference's (above), so this is the model of the reference's samples
+    kind = {pb.PB2_FILTER_BOX: "box", pb.PB2_FILTER_GAUSSIAN: "gaussian", pb.PB2_FILTER_MITCHELL: "mitchell", pb.PB2_FILTER_SINC: "sinc",
+            pb.PB2_FILTER_TRIANGLE: "triangle"}[film.filter_type]
+    assert kind in MODELLED_FILTERS
+    # the samples equal the reference's (above), so this is the model of the reference's samples; the bound takes |L * w|,
+    # so the negative lobes of the mitchell and sinc filters are covered
     model, bound = film_model(film, li, pfilm)
     for name, f in (("shipped", shipped), ("PB2_FINISH=0", rounds[case + ":film"])):
         why = model_mismatch(f, model, bound, kind == "box")

@@ -77,18 +77,26 @@ CONFIGS = {
 }
 
 
+def case_text(case):
+    """The scene text of this file's own cases (the others: test_gpu_wavefront_schedules.case_text)."""
+    if case == "matte_box":
+        return MATTE_BOX
+    if case == "matte_mesh_lights":
+        from test_gpu_parity import emissive_mesh_scene
+        text = emissive_mesh_scene(40)
+        assert text.count('Material "plastic"') == 1
+        return text.replace('Material "plastic"', 'Material "matte"')
+    import test_gpu_wavefront_schedules as ws
+    return ws.case_text(case)
+
+
 def make_case(pb, case):
     if case == "killeroo_simple":
         import argparse
         import bench
         return bench.build_scene(argparse.Namespace(workload="killeroo", xres=32, yres=18, spp=1, maxdepth=5))
-    if case == "matte_box":
-        return pb.HostScene.from_string(MATTE_BOX)
-    if case == "matte_mesh_lights":
-        from test_gpu_parity import emissive_mesh_scene
-        text = emissive_mesh_scene(40)
-        assert text.count('Material "plastic"') == 1
-        return pb.HostScene.from_string(text.replace('Material "plastic"', 'Material "matte"'))
+    if case in ("matte_box", "matte_mesh_lights"):
+        return pb.HostScene.from_string(case_text(case))
     import test_gpu_wavefront_schedules as ws
     return ws.make_case(pb, case)
 

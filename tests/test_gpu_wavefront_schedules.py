@@ -11,8 +11,9 @@ Checks:
   1. per-pixel model: every work item's L and pFilm from pb2_li_samples (one thread per sample, the same lane functions),
      clamped like addSample and deposited in float64 with FilmTile::AddSample's pixel range.  The weight channel of a
      box-filtered film must equal the model's exactly; every RGB value must lie within k * 2^-24 * sum |L * w| of the
-     model, k = deposits in the pixel: the error bound of float32 additions in any order.  This assumes a path's L is
-     bit-identical in the wavefront and in pb2_li_samples (both run the same functions under -fmad=false).
+     model, k = deposits in the pixel: the error bound of float32 additions in any order.  This rests on a path's L being
+     bit-identical in the wavefront and in pb2_li_samples, which tests/test_gpu_sample_films.py checks: at one sample per
+     pixel the film holds each path's L itself, in every schedule and configuration of this file.
   2. ray counters: camera rays = valid work items; regular and shadow rays equal in every schedule and under every flag.
   3. the golden scenes at native spp, with the rounds forced, against the reference's image and ray counts.
   4. PB2_FLAG_CHAIN: checks 1-3 everywhere, fewer launches, and the reference's emissive-sphere furnace.
@@ -95,24 +96,29 @@ WorldEnd
 """
 
 
-def make_case(pb, case):
+def case_text(case):
+    """The scene text of a case that is not a golden scene file or a synthetic generator."""
     from test_gpu_parity import emissive_mesh_scene
+    if case == "lights_spatial_lazy":
+        return gc.lights_text(SCENES, "spatial")
+    if case == "emissive_mesh":
+        return emissive_mesh_scene(40)          # 3200 lights: the spatial table is built on demand
+    if case == "emissive_sphere":
+        return gc.analytic_scene_text("emissive_sphere")
+    if case == "gaussian":
+        return gc.filter_scene_text(SCENES, "gaussian")
+    if case == "one_sided_lights":
+        return ONE_SIDED_LIGHTS
+    raise KeyError(case)
+
+
+def make_case(pb, case):
     from test_oracle import load_scene
     if case in GOLDEN_CASES:
         return load_scene(pb, case)
-    if case == "lights_spatial_lazy":
-        return pb.HostScene.from_string(gc.lights_text(SCENES, "spatial"))
-    if case == "emissive_mesh":
-        return pb.HostScene.from_string(emissive_mesh_scene(40))          # 3200 lights: the spatial table is built on demand
-    if case == "emissive_sphere":
-        return pb.HostScene.from_string(gc.analytic_scene_text("emissive_sphere"))
     if case == "instanced_soup":
         return pb.HostScene.instanced_soup(2000, grid=4, xres=64, yres=36, spp=4)
-    if case == "gaussian":
-        return pb.HostScene.from_string(gc.filter_scene_text(SCENES, "gaussian"))
-    if case == "one_sided_lights":
-        return pb.HostScene.from_string(ONE_SIDED_LIGHTS)
-    raise KeyError(case)
+    return pb.HostScene.from_string(case_text(case))
 
 
 def case_flags(pb, case):
@@ -127,65 +133,117 @@ def case_flags(pb, case):
 # The per-pixel model (host arithmetic only)
 # ---------------------------------------------------------------------------------------------------------------------
 def filter_table(film):
-    """Film's 16 x 16 filter weight table as the library's host code builds it (float arithmetic, libm's expf), or None
-    for the box filter.  Only the box and the gaussian filter are modelled."""
+    """Film's 16 x 16 filter weight table as the library's host code builds it (computeFilterTable: Filter::Evaluate in
+    float, in the same order, with libm's expf and sinf), or None for the box filter."""
     import pbrt_v3_b200 as pb
     if film.filter_type == pb.PB2_FILTER_BOX:
         return None
-    if film.filter_type != pb.PB2_FILTER_GAUSSIAN:
-        raise NotImplementedError("filter type %d is not modelled" % film.filter_type)
     libm = C.CDLL(ctypes.util.find_library("m"))
     libm.expf.restype, libm.expf.argtypes = C.c_float, [C.c_float]
+    libm.sinf.restype, libm.sinf.argtypes = C.c_float, [C.c_float]
     f32 = np.float32
     expf = lambda v: f32(libm.expf(float(v)))
-    rx, ry, alpha = f32(film.filter_radius[0]), f32(film.filter_radius[1]), f32(film.filter_param[0])
-    exp_x, exp_y = expf(-alpha * rx * rx), expf(-alpha * ry * ry)
-    g = lambda d, e: max(f32(0), f32(expf(-alpha * d * d) - e))
+    sinf = lambda v: f32(libm.sinf(float(v)))
+    rx, ry = f32(film.filter_radius[0]), f32(film.filter_radius[1])
+    p0, p1 = f32(film.filter_param[0]), f32(film.filter_param[1])
+    if film.filter_type == pb.PB2_FILTER_GAUSSIAN:           # gaussian.h:50-66
+        alpha = p0
+        exp_x, exp_y = expf(-alpha * rx * rx), expf(-alpha * ry * ry)
+        g = lambda d, e: max(f32(0), f32(expf(-alpha * d * d) - e))
+        evaluate = lambda x, y: g(x, exp_x) * g(y, exp_y)
+    elif film.filter_type == pb.PB2_FILTER_MITCHELL:         # mitchell.h:53-63
+        B, Cm = p0, p1
+
+        def m1(v):
+            v = abs(f32(2) * v)
+            if v > f32(1):
+                return ((-B - f32(6) * Cm) * v * v * v + (f32(6) * B + f32(30) * Cm) * v * v + (f32(-12) * B - f32(48) * Cm) * v
+                        + (f32(8) * B + f32(24) * Cm)) * (f32(1) / f32(6))
+            return ((f32(12) - f32(9) * B - f32(6) * Cm) * v * v * v + (f32(-18) + f32(12) * B + f32(6) * Cm) * v * v
+                    + (f32(6) - f32(2) * B)) * (f32(1) / f32(6))
+        inv_rx, inv_ry = f32(1) / rx, f32(1) / ry
+        evaluate = lambda x, y: m1(x * inv_rx) * m1(y * inv_ry)
+    elif film.filter_type == pb.PB2_FILTER_SINC:             # sinc.h:53-63
+        tau, pi = p0, f32(3.14159265358979323846)
+
+        def sinc(v):
+            v = abs(v)
+            if float(v) < 1e-5:                                  # a float against a double literal
+                return f32(1)
+            return sinf(pi * v) / (pi * v)
+
+        def windowed(v, radius):
+            v = abs(v)
+            if v > radius:
+                return f32(0)
+            lanczos = sinc(v / tau)
+            return sinc(v) * lanczos
+        evaluate = lambda x, y: windowed(x, rx) * windowed(y, ry)
+    elif film.filter_type == pb.PB2_FILTER_TRIANGLE:         # triangle.cpp:40-43
+        evaluate = lambda x, y: max(f32(0), rx - abs(x)) * max(f32(0), ry - abs(y))
+    else:
+        raise NotImplementedError("filter type %d is not modelled" % film.filter_type)
     table = np.zeros(256, np.float32)
     for y in range(16):
         for x in range(16):
-            table[y * 16 + x] = g((f32(x) + f32(.5)) * rx / f32(16), exp_x) * g((f32(y) + f32(.5)) * ry / f32(16), exp_y)
+            table[y * 16 + x] = evaluate((f32(x) + f32(.5)) * rx / f32(16), (f32(y) + f32(.5)) * ry / f32(16))
     return table
 
 
-def film_model(film, li, pfilm):
-    """The film that depositing the samples (li, pfilm) must give: addSample's maxSampleLuminance clamp in float32, then
-    FilmTile::AddSample's pixel range and filter-table look-up in float32 and the sum in float64.  Returns (rgbw, bound):
-    rgbw (h, w, 4) float64, bound (h, w, 4) = k * 2^-24 * sum |L * w| per channel, k = deposits in the pixel."""
+def clamped_samples(film, li):
+    """L as addSample deposits it: scaled down to maxSampleLuminance where its luminance is above it (float32)."""
     f32 = np.float32
-    x0, y0, x1, y1 = (int(v) for v in film.cropped_pixel_bounds)
-    h, w = y1 - y0, x1 - x0
     L = np.array(li, np.float32)
     lum = f32(0.212671) * L[:, 0] + f32(0.715160) * L[:, 1] + f32(0.072169) * L[:, 2]
     m = f32(film.max_sample_luminance)
     over = lum > m
     L[over] = L[over] * (m / lum[over])[:, None]
-    table = filter_table(film)
+    return L
+
+
+def deposits(film, pfilm):
+    """FilmTile::AddSample's pixel range of every sample, clipped to the cropped bounds: yields (sample indices, pixel x,
+    pixel y, filter-table index) once per offset inside the ranges (the table index is None for the box filter)."""
+    f32 = np.float32
+    x0, y0, x1, y1 = (int(v) for v in film.cropped_pixel_bounds)
+    box = filter_table(film) is None
     rx, ry = f32(film.filter_radius[0]), f32(film.filter_radius[1])
     inv_rx, inv_ry = f32(1) / rx, f32(1) / ry
     pf = np.asarray(pfilm, np.float32)
     dx, dy = pf[:, 0] - f32(.5), pf[:, 1] - f32(.5)
     p0x, p0y = np.maximum(np.ceil(dx - rx).astype(np.int64), x0), np.maximum(np.ceil(dy - ry).astype(np.int64), y0)
     p1x, p1y = np.minimum(np.floor(dx + rx).astype(np.int64) + 1, x1), np.minimum(np.floor(dy + ry).astype(np.int64) + 1, y1)
-    total = np.zeros((h * w, 4), np.float64)
-    absum = np.zeros((h * w, 4), np.float64)
-    k = np.zeros(h * w, np.float64)
     for oy in range(max(0, int((p1y - p0y).max(initial=0)))):
         for ox in range(max(0, int((p1x - p0x).max(initial=0)))):
             xx, yy = p0x + ox, p0y + oy
-            sel = (xx < p1x) & (yy < p1y)
+            sel = np.flatnonzero((xx < p1x) & (yy < p1y))
             xs, ys = xx[sel], yy[sel]
-            if table is None:
-                wt = np.ones(len(xs), np.float32)
-            else:
+            tab = None
+            if not box:
                 fx = np.abs((xs.astype(np.float32) - dx[sel]) * inv_rx * f32(16))
                 fy = np.abs((ys.astype(np.float32) - dy[sel]) * inv_ry * f32(16))
-                wt = table[np.minimum(np.floor(fy).astype(np.int64), 15) * 16 + np.minimum(np.floor(fx).astype(np.int64), 15)]
-            contrib = np.concatenate([L[sel] * wt[:, None], wt[:, None]], 1).astype(np.float64)
-            idx = (ys - y0) * w + (xs - x0)
-            np.add.at(total, idx, contrib)
-            np.add.at(absum, idx, np.abs(contrib))
-            np.add.at(k, idx, 1)
+                tab = np.minimum(np.floor(fy).astype(np.int64), 15) * 16 + np.minimum(np.floor(fx).astype(np.int64), 15)
+            yield sel, xs, ys, tab
+
+
+def film_model(film, li, pfilm):
+    """The film that depositing the samples (li, pfilm) must give: addSample's maxSampleLuminance clamp in float32, then
+    FilmTile::AddSample's pixel range and filter-table look-up in float32 and the sum in float64.  Returns (rgbw, bound):
+    rgbw (h, w, 4) float64, bound (h, w, 4) = k * 2^-24 * sum |L * w| per channel, k = deposits in the pixel."""
+    x0, y0, x1, y1 = (int(v) for v in film.cropped_pixel_bounds)
+    h, w = y1 - y0, x1 - x0
+    L = clamped_samples(film, li)
+    table = filter_table(film)
+    total = np.zeros((h * w, 4), np.float64)
+    absum = np.zeros((h * w, 4), np.float64)
+    k = np.zeros(h * w, np.float64)
+    for sel, xs, ys, tab in deposits(film, pfilm):
+        wt = np.ones(len(xs), np.float32) if table is None else table[tab]
+        contrib = np.concatenate([L[sel] * wt[:, None], wt[:, None]], 1).astype(np.float64)
+        idx = (ys - y0) * w + (xs - x0)
+        np.add.at(total, idx, contrib)
+        np.add.at(absum, idx, np.abs(contrib))
+        np.add.at(k, idx, 1)
     return total.reshape(h, w, 4), (k[:, None] * U * absum).reshape(h, w, 4)
 
 
@@ -382,11 +440,12 @@ def test_tile_partition_sums_to_the_model(schedule, name, case):
 # ---------------------------------------------------------------------------------------------------------------------
 # The model itself, on the CPU: the oracle port's samples through it give the port's own render
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("case", ["soup", "gaussian"])
+@pytest.mark.parametrize("case", ["soup"] + list(gc.FILTER_CASES))
 def test_model_reproduces_the_port_render(port, case):
+    """Every reconstruction filter of golden_cases.FILTER_CASES ("gaussian" is also this file's gaussian case)."""
     import pbrt_v3_b200 as pb
     from pbrt_v3_b200 import multigpu
-    hs = make_case(pb, case)
+    hs = make_case(pb, case) if case in CASES else pb.HostScene.from_string(gc.filter_scene_text(SCENES, case))
     sc = port.scene(hs)
     items = multigpu.work_items(hs.film, hs.params)
     li, pfilm = sc.li_samples(items[:, :2], items[:, 2].astype(np.int64))
@@ -394,5 +453,15 @@ def test_model_reproduces_the_port_render(port, case):
     want, _, _ = sc.render(n_threads=1)
     got = hs.resolve(model.astype(np.float32))
     rel = np.abs(got - want) / np.maximum(np.abs(want), 1e-3)
+    table = filter_table(hs.film.contents)
+    if table is not None and (table < 0).any():
+        # negative lobes (mitchell, sinc): where they nearly cancel, the port's own float32 sums are off by up to their
+        # bounds relative to the small sums that remain.  Such values may exceed 1e-5 by that much, and only a few may
+        # (1 of the 13 440 values of the four cases does, the sinc case's).
+        part = lambda b, m: b / np.maximum(np.abs(m), 1e-30)
+        allowance = (part(bound[..., :3], model[..., :3]) + part(bound[..., 3:], model[..., 3:])) * np.abs(want) / np.maximum(np.abs(want), 1e-3)
+        loose = rel > 1e-5
+        assert loose.sum() <= rel.size // 1000, int(loose.sum())
+        rel = np.where(loose, rel - allowance, rel)
     assert rel.max() <= 1e-5, float(rel.max())
     assert (model[..., 3] > 0).all() and (bound >= 0).all()
