@@ -83,42 +83,40 @@ PB2_HD void startMisOrFinish(DLane &ln) {
         finishVertex(ln);
 }
 
-// The path ray has been traced: one iteration of the bounce loop up to (not including) the results
-// of the two direct-lighting rays.
-// LAZY = false compiles the deferral of the lazy light distribution out (the bench scene's shade kernel sits exactly at
-// its 128-register budget)
-// TEX = true is the GENERAL instantiation: it evaluates image textures (tc then carries what the camera ray's differentials
-// are rebuilt from) and draws from the SobolSampler when the frame uses it (sampleDimension<true>).
+// What the camera ray's differentials are rebuilt from when image textures are evaluated.
 struct DTexCtx {
     const DCamera *cam;
     V2 pFilm;           // of this camera sample
     float diffScale;    // 1 / sqrt(samples per pixel)
 };
 
+// The path ray has been traced: one iteration of the bounce loop up to (not including) the results
+// of the two direct-lighting rays.
+// F: the shade features (SHADE_* in pb2_shade.cuh) the vertex is compiled for.
 // u: room for the vertex's kSampleBatch sampler values (the caller's: shared memory in the shade step).
-// FC: the scene's shade feature class (SHADE_* in pb2_shade.cuh), SHADE_ALL when it is not known.
-template <bool SPH, bool SPEC = true, bool LAZY = true, bool TEX = false, int FC = SHADE_ALL>
+template <int F>
 PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &pp, DLane &ln, bool found, const DHit &hit,
                         float tMax, float *u, const DTexCtx *tc = nullptr) {
+    constexpr bool SOBOL = (F & SHADE_SOBOL) != 0;
     // Every dimension this vertex can draw, [smp.dim, smp.dim + kSampleBatch), evaluated up front: the values are a pure
     // function of (index, dimension), and drawn here their table loads overlap the hit's leaf-record loads instead of
     // forming a chain of round trips each where its value is used.  A vertex that draws nothing skips it.
     const int dim0 = ln.smp.dim;
-    if (found && ln.bounces < pp.maxDepth) haltonSampleBatch<TEX>(h, ln.smp.index, dim0, kSampleBatch, u);
+    if (found && ln.bounces < pp.maxDepth) haltonSampleBatch<SOBOL>(h, ln.smp.index, dim0, kSampleBatch, u);
     DInteraction isect;
     int li = -1;
     DTexGeom tg;
     DUvDiff uvDiff;
     uvDiff.dudx = uvDiff.dvdx = uvDiff.dudy = uvDiff.dvdy = 0;
-    if (found) isect = hitInteraction<SPH>(sc, hit, ln.ray, tMax, &li, (TEX && tc) ? &tg : nullptr);
-    if (TEX && tc && sc.textures) {
+    if (found) isect = hitInteraction<F>(sc, hit, ln.ray, tMax, &li, ((F & SHADE_TEXTURES) && tc) ? &tg : nullptr);
+    if ((F & SHADE_TEXTURES) && tc && sc.textures) {
         if (found && ln.camRay) {
             // the camera ray's differentials are a pure function of the camera sample: rebuilt here, not carried in the lane
             V2 uLens = mk2(0, 0);
             if (tc->cam->lensRadius > 0) {
                 DSampler ls = ln.smp;
                 ls.dim = 3;   // CameraSample::pLens (sampler.cpp:46-52)
-                uLens = get2D<TEX>(h, ls);
+                uLens = get2D<SOBOL>(h, ls);
             }
             const DRayDiff rd = cameraRayDifferentials(*tc->cam, tc->pFilm, uLens, tc->diffScale, ln.ray.o, ln.ray.d);
             uvDiff = computeUvDifferentials(isect.p, isect.n, tg.dpdu, tg.dpdv, rd);
@@ -131,7 +129,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
         }
     }
     const float *lazyDistrib = nullptr;
-    if (LAZY && sc.lightDist.slots && found && ln.bounces < pp.maxDepth) {
+    if ((F & SHADE_LAZY) && sc.lightDist.slots && found && ln.bounces < pp.maxDepth) {
         // lazy light distribution: look the voxel up before anything of the lane changes, so that a miss can hand the
         // vertex back untouched (the record is a pure function of the voxel: when it is built does not matter)
         lazyDistrib = lightDistLookup(sc.lightDist, isect.p);
@@ -145,7 +143,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             if (li >= 0) ln.L = ln.L + ln.beta * lightL(sc.lights[li], isect.n, -ln.ray.d);
         } else {
             // the ray escaped: every infinite light is seen directly (path.cpp:96-98)
-            if (FC & SHADE_NON_AREA)
+            if (F & SHADE_NON_AREA)
                 for (int k = 0; k < sc.nInfinite; ++k)
                     ln.L = ln.L + ln.beta * infiniteLe(sc, sc.lights[sc.infinite[k]], sc.deltaLights[sc.infinite[k]], ln.ray.d);
         }
@@ -154,13 +152,13 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
         ln.state = LS_IDLE;
         return;
     }
-    if (TEX) ln.camRay = false;   // every ray spawned from here on is a plain Ray
+    if (F & SHADE_TEXTURES) ln.camRay = false;   // every ray spawned from here on is a plain Ray
     DBsdf bsdf;
-    if (!makeBsdf<SPEC, TEX, FC>(sc, isect, &bsdf, TEX ? &uvDiff : nullptr)) {
+    if (!makeBsdf<F>(sc, isect, &bsdf, (F & SHADE_TEXTURES) ? &uvDiff : nullptr)) {
         ln.ray = spawnRay(isect, ln.ray.d);  // null BSDF: skip the surface, same bounce count
         return;
     }
-    const float *distrib = (LAZY && lazyDistrib) ? lazyDistrib : lightDistLookup(sc.lightDist, isect.p);
+    const float *distrib = ((F & SHADE_LAZY) && lazyDistrib) ? lazyDistrib : lightDistLookup(sc.lightDist, isect.p);
     // The lane lives in HBM and is updated in place, the sampler's dimension counter included (a
     // register copy of ln.smp across this function would not fit: the 128-register budget is full).
     DSampler &smp = ln.smp;
@@ -176,20 +174,20 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
     if (ln.doNEE && sc.nLights > 0) {
         // UniformSampleOneLight (integrator.cpp:85-106)
         float lightPickPdf;
-        int lightNum = sampleDiscrete(distrib, sc.nLights, get1D<TEX>(h, smp, u, dim0), &lightPickPdf);
+        int lightNum = sampleDiscrete(distrib, sc.nLights, get1D<SOBOL>(h, smp, u, dim0), &lightPickPdf);
         if (lightPickPdf != 0) {
             ln.pick = lightPickPdf;
             ln.lightNum = lightNum;
             const pb2_light light = sc.lights[lightNum];
             const TriRec lightRec = loadTriRec(sc.lightRecs, (size_t)lightNum);
-            V2 uLight = get2D<TEX>(h, smp, u, dim0);
-            V2 uScattering = get2D<TEX>(h, smp, u, dim0);
+            V2 uLight = get2D<SOBOL>(h, smp, u, dim0);
+            V2 uScattering = get2D<SOBOL>(h, smp, u, dim0);
             // EstimateDirect, light-sampling half (integrator.cpp:116-160)
-            DLightSample ls = sampleLight<SPH, FC>(sc, lightNum, light, lightRec, isect, uLight);
+            DLightSample ls = sampleLight<F>(sc, lightNum, light, lightRec, isect, uLight);
             float lightPdf = ls.pdf, scatteringPdf = 0;
             if (lightPdf > 0 && !isBlack(ls.Li)) {
-                V3 f = bsdfF<SPEC, FC>(bsdf, isect.wo, ls.wi) * absDot(ls.wi, isect.ns);
-                scatteringPdf = bsdfPdf<SPEC, FC>(bsdf, isect.wo, ls.wi);
+                V3 f = bsdfF<F>(bsdf, isect.wo, ls.wi) * absDot(ls.wi, isect.ns);
+                scatteringPdf = bsdfPdf<F>(bsdf, isect.wo, ls.wi);
                 if (!isBlack(f)) {
                     shadow = spawnRayTo(isect, ls.p, ls.pError, ls.n);
                     hasShadow = true;
@@ -203,19 +201,19 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             V3 wi;
             V3 f = mk3(0, 0, 0);
             if (!ls.delta) {
-                f = bsdfSampleF<SPEC, FC>(bsdf, isect.wo, &wi, uScattering, &scatteringPdf, nullptr, true);
+                f = bsdfSampleF<F>(bsdf, isect.wo, &wi, uScattering, &scatteringPdf, nullptr, true);
                 if (scatteringPdf != 0) f = f * absDot(wi, isect.ns);
                 else f = mk3(0, 0, 0);
             }
             if (!isBlack(f) && scatteringPdf > 0) {
-                lightPdf = lightPdfLi<SPH, FC>(sc, light, lightRec, isect, wi, lightNum);
+                lightPdf = lightPdfLi<F>(sc, light, lightRec, isect, wi, lightNum);
                 if (lightPdf != 0) {
                     float weight = powerHeuristic(scatteringPdf, lightPdf);
                     // Li is the light's Lemit when the MIS ray reaches its emitting side (checked after
                     // the trace); f * Li * Tr(=1) * weight / scatteringPdf.  An infinite light is seen when the ray
                     // escapes instead (integrator.cpp:209-211): its Le along wi is known here already.
                     V3 Lmis = mk3(light.L[0], light.L[1], light.L[2]);
-                    if ((FC & SHADE_NON_AREA) && sc.deltaLights && light.type == PB2_LIGHT_INFINITE) Lmis = infiniteLe(sc, light, sc.deltaLights[lightNum], wi);
+                    if ((F & SHADE_NON_AREA) && sc.deltaLights && light.type == PB2_LIGHT_INFINITE) Lmis = infiniteLe(sc, light, sc.deltaLights[lightNum], wi);
                     V3 fl = f * Lmis * weight;
                     ln.misTerm = mk3(fl.x / scatteringPdf, fl.y / scatteringPdf, fl.z / scatteringPdf);
                     DRay mr = spawnRay(isect, wi);
@@ -233,7 +231,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
         V3 wo = -ln.ray.d, wi;
         float pdf;
         int sampled = 0;
-        V3 f = bsdfSampleF<SPEC, FC>(bsdf, wo, &wi, get2D<TEX>(h, smp, u, dim0), &pdf, &sampled);
+        V3 f = bsdfSampleF<F>(bsdf, wo, &wi, get2D<SOBOL>(h, smp, u, dim0), &pdf, &sampled);
         if (!(isBlack(f) || pdf == 0.f)) {
             V3 s = f * absDot(wi, isect.ns);
             V3 beta = ln.beta * mk3(s.x / pdf, s.y / pdf, s.z / pdf);
@@ -248,7 +246,7 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
             V3 rrBeta = beta * ln.etaScale;
             if (maxComponentValue(rrBeta) < pp.rrThreshold && ln.bounces > 3) {
                 float q = pmax(.05f, 1 - maxComponentValue(rrBeta));
-                if (get1D<TEX>(h, smp, u, dim0) < q) survive = false;
+                if (get1D<SOBOL>(h, smp, u, dim0) < q) survive = false;
                 else {
                     float d = 1 - q;
                     beta = mk3(beta.x / d, beta.y / d, beta.z / d);
@@ -271,9 +269,9 @@ PB2_HD void shadeVertex(const DScene &sc, const DHalton &h, const DPathParams &p
 }
 
 // A shadow or MIS ray has been traced: add its term, then start the vertex's next ray or finish it.
-template <bool SPH, int FC = SHADE_ALL>
+template <int F>
 PB2_HD void lightAdvance(const DScene &sc, DLane &ln, bool found, const DHit &hit, float tMax) {
-    const bool nonArea = (FC & SHADE_NON_AREA) && sc.deltaLights;
+    const bool nonArea = (F & SHADE_NON_AREA) && sc.deltaLights;
     if (ln.state == LS_SHADOW) {
         if (!found) ln.ldSum = ln.ldSum + ln.ldLight;  // VisibilityTester::Unoccluded
         startMisOrFinish(ln);
@@ -285,13 +283,13 @@ PB2_HD void lightAdvance(const DScene &sc, DLane &ln, bool found, const DHit &hi
             // the hit primitive's light number rides in its leaf record (spheres: via primLight)
             float4 b = ldg4(&sc.leafPrims[3 * (size_t)hit.leaf + 1]), c = ldg4(&sc.leafPrims[3 * (size_t)hit.leaf + 2]);
             int hitLight = asInt(c.w);
-            if (SPH && (floatBits(b.w) & LEAF_SPHERE)) hitLight = sc.primLight[asInt(ldg4(&sc.leafPrims[3 * (size_t)hit.leaf]).w)];
+            if ((F & SHADE_SPHERES) && (floatBits(b.w) & LEAF_SPHERE)) hitLight = sc.primLight[asInt(ldg4(&sc.leafPrims[3 * (size_t)hit.leaf]).w)];
             if (hitLight == ln.lightNum) {
                 const pb2_light light = sc.lights[ln.lightNum];
                 // lightIsect.Le(-wi): DiffuseAreaLight::L with the hit's (face-forwarded) normal
                 if (light.two_sided) ln.ldSum = ln.ldSum + ln.misTerm;
                 else {
-                    DInteraction lightIsect = hitInteraction<SPH>(sc, hit, ln.ray, tMax);
+                    DInteraction lightIsect = hitInteraction<F>(sc, hit, ln.ray, tMax);
                     if (dot(lightIsect.n, -ln.ray.d) > 0) ln.ldSum = ln.ldSum + ln.misTerm;
                 }
             }
@@ -301,15 +299,15 @@ PB2_HD void lightAdvance(const DScene &sc, DLane &ln, bool found, const DHit &hi
 }
 
 // Advance a lane after its current ray was traced.  Returns true when the path ended in this call
-// (ln.L is then final and ln.state == LS_IDLE).
-template <bool SPH, bool SPEC = true, bool TEX = false, int FC = SHADE_ALL>
+// (ln.L is then final and ln.state == LS_IDLE).  The vertex can always be handed back (SHADE_LAZY): the caller checks LS_DEFER.
+template <int F>
 PB2_HD bool laneAdvance(const DScene &sc, const DHalton &h, const DPathParams &pp, DLane &ln, bool found, const DHit &hit,
                         float tMax, const DTexCtx *tc = nullptr) {
     if (ln.state == LS_PATH) {
         float u[kSampleBatch];
-        shadeVertex<SPH, SPEC, true, TEX, FC>(sc, h, pp, ln, found, hit, tMax, u, tc);
+        shadeVertex<F | SHADE_LAZY>(sc, h, pp, ln, found, hit, tMax, u, tc);
     } else
-        lightAdvance<SPH, FC>(sc, ln, found, hit, tMax);
+        lightAdvance<F>(sc, ln, found, hit, tMax);
     return ln.state == LS_IDLE;
 }
 

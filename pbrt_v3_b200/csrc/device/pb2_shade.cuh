@@ -202,13 +202,27 @@ PB2_HD DInteraction triangleInteraction(const DScene &sc, const TriRec &rec, flo
 
 namespace pb2 {
 
-// SPH = false compiles the sphere branches away (scenes without spheres get kernels without the
-// interval-arithmetic code and its call frames).
+// Shade features (the F template argument of the path functions and kernels): what a frame's scene records and parameters
+// can reach.  A bit that is clear compiles away the branches whose run-time condition is false for every record of the
+// scene and every parameter of the frame; the code that remains is the same, in the same order.  The host computes a
+// frame's mask (frameShadeFeatures in pb2_cuda.cu) and runs the kernel compiled for the fewest bits that contain it.
+//   SHADE_OREN_NAYAR   a matte material with sigma != 0 (diffuseKind 2)
+//   SHADE_MICROFACET   a plastic material (its Trowbridge-Reitz lobe, hasMicrofacet)
+//   SHADE_NON_AREA     a point, spot, distant or infinite light (DScene::deltaLights, nInfinite)
+//   SHADE_SPHERES      sphere primitives and sphere area lights (LEAF_SPHERE; the interval-arithmetic code and its call frames)
+//   SHADE_SPECULAR     a mirror, glass, substrate, metal or uber material (specKind, blend, general)
+//   SHADE_LAZY         the lazy light distribution (DLightDist::slots): a vertex can be handed back (LS_DEFER)
+//   SHADE_TEXTURES     image textures: materials' texture slots and bump maps, and the camera ray's differentials
+//   SHADE_SOBOL        the frame draws from the SobolSampler (the sampler functions' GENERAL)
+// The first three are the shade class that pb2_shade_class reports; SHADE_GENERAL is the class with every lobe and light.
+enum { SHADE_OREN_NAYAR = 1, SHADE_MICROFACET = 2, SHADE_NON_AREA = 4, SHADE_SPHERES = 8, SHADE_SPECULAR = 16, SHADE_LAZY = 32,
+       SHADE_TEXTURES = 64, SHADE_SOBOL = 128, SHADE_LAMBERT_AREA = 0, SHADE_GENERAL = 7, SHADE_FULL = 255 };
+
 // *light receives the area-light number of the primitive that was hit (-1: not emissive).
 // A hit inside an instanced object was found with the ray in instance space (hit.inst >= 0): the
 // interaction is built there and then taken to world space as TransformedPrimitive::Intersect does
 // with Transform::operator()(const SurfaceInteraction &) (primitive.cpp:85-86, transform.cpp:262-297).
-template <bool SPH = true>
+template <int F>
 PB2_HD DInteraction hitInteraction(const DScene &sc, const DHit &hit, const DRay &ray, float tHit, int *light = nullptr, DTexGeom *tg = nullptr) {
     TriRec rec = loadTriRec(sc.leafPrims, (size_t)hit.leaf);
     const DInstance *inst = nullptr;
@@ -218,7 +232,7 @@ PB2_HD DInteraction hitInteraction(const DScene &sc, const DHit &hit, const DRay
         r = xfRay(inst->w2i, ray, ray.tMax);
     }
     DInteraction it;
-    if (SPH && (rec.flags & LEAF_SPHERE)) {
+    if ((F & SHADE_SPHERES) && (rec.flags & LEAF_SPHERE)) {
         if (light) *light = sc.primLight[rec.prim];
         it = sphereInteraction(sc, rec.prim, r, tHit, hit.b0, tg);
     } else {
@@ -289,14 +303,6 @@ struct DBsdf {
     float e;               // the index the lobes' Fresnel terms use (BSDF::eta is 1 when GEN_OPACITY is present)
 };
 enum { BSDF_SAMPLED_SPECULAR = 1, BSDF_SAMPLED_TRANSMISSION = 2 };
-// A shade feature class (the FC template argument of the BSDF, light and lane functions): the lobes and lights that the
-// scene's material and light records can produce among those of the non-specular materials' BSDFs and the area lights.
-// A bit that is clear compiles away a branch whose run-time condition is false for every record of such a scene; the
-// code that remains is the same, in the same order.  The host picks the class (shadeFeatureClass in pb2_cuda.cu).
-//   SHADE_OREN_NAYAR   a matte material with sigma != 0 (diffuseKind 2)
-//   SHADE_MICROFACET   a plastic material (its Trowbridge-Reitz lobe, hasMicrofacet)
-//   SHADE_NON_AREA     a point, spot, distant or infinite light (DScene::deltaLights, nInfinite)
-enum { SHADE_OREN_NAYAR = 1, SHADE_MICROFACET = 2, SHADE_NON_AREA = 4, SHADE_ALL = 7, SHADE_LAMBERT_AREA = 0 };
 enum { GEN_OPACITY = 1, GEN_LAMBERT = 2, GEN_MICROFACET = 4, GEN_SPEC_REFLECTION = 8, GEN_SPEC_TRANSMISSION = 16,
        GEN_MICRO_TRANSMISSION = 32,   // MicrofacetTransmission(specT, TrowbridgeReitz(alphaX, alphaY), 1, e): rough glass
        GEN_LOBES = 6, GEN_NON_SPECULAR = GEN_LAMBERT | GEN_MICROFACET | GEN_MICRO_TRANSMISSION };
@@ -312,9 +318,6 @@ PB2_HD float roughnessToAlpha(float roughness) {
     return 1.62142f + 0.819955f * x + 0.1734f * x * x + 0.0171201f * x * x * x + 0.000640711f * x * x * x * x;
 }
 
-// Material::ComputeScatteringFunctions for matte (matte.cpp:45-62) and plastic (plastic.cpp:45-70).
-// Returns false when the primitive has no material (null BSDF: the path skips the surface).
-// SPEC = false compiles the specular materials away (scenes without mirror / glass get the leaner kernel).
 // The textured parameters of a material at one shaded point: every slot of pb2_material::tex that names a texture is
 // evaluated (Texture::Evaluate(*si), e.g. matte.cpp:53-54) and written over the constant.
 PB2_HDN void applyTextures(const DScene &sc, V2 uv, const DUvDiff &d, pb2_material *mat) {
@@ -363,14 +366,16 @@ PB2_HDN void bumpShading(const DScene &sc, int tex, const DTexGeom &tg, const DU
     it->dpdus = dpdu;
 }
 
-// TEX = true: image textures are evaluated (uvDiff: the point's (u, v) differentials); false compiles them away.
-template <bool SPEC = true, bool TEX = false, int FC = SHADE_ALL>
+// Material::ComputeScatteringFunctions for matte (matte.cpp:45-62) and plastic (plastic.cpp:45-70).
+// Returns false when the primitive has no material (null BSDF: the path skips the surface).
+// uvDiff: the point's (u, v) differentials, which image textures are evaluated with.
+template <int F>
 PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, const DUvDiff *uvDiff = nullptr) {
     int m = sc.primMaterial[it.prim];
     if (m < 0) return false;
     pb2_material mat = sc.materials[m];
     if (mat.type == PB2_MAT_NONE) return false;
-    if (TEX && sc.textures && uvDiff) applyTextures(sc, it.uv, *uvDiff, &mat);
+    if ((F & SHADE_TEXTURES) && sc.textures && uvDiff) applyTextures(sc, it.uv, *uvDiff, &mat);
     bsdf->ns = it.ns;
     bsdf->ng = it.n;
     bsdf->ss = normalize(it.dpdus);
@@ -391,7 +396,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
     bsdf->conductor = 0;
     bsdf->T0 = bsdf->condEta = bsdf->condK = mk3(0, 0, 0);
     bsdf->e = 1;
-    if (SPEC && mat.type == PB2_MAT_METAL) {
+    if ((F & SHADE_SPECULAR) && mat.type == PB2_MAT_METAL) {
         // metal.cpp:60-80: one MicrofacetReflection(1, TrowbridgeReitz(uRough, vRough), FresnelConductor(1, eta, k))
         float uRough = mat.uroughness, vRough = mat.vroughness;
         if (mat.remap_roughness) {
@@ -408,7 +413,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         bsdf->nLobes = 1;
         return true;
     }
-    if (SPEC && mat.type == PB2_MAT_UBER) {
+    if ((F & SHADE_SPECULAR) && mat.type == PB2_MAT_UBER) {
         // uber.cpp:45-104
         const float e = mat.eta;
         V3 op = clampSpectrum(mat.opacity);
@@ -451,7 +456,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         }
         return true;
     }
-    if (SPEC && mat.type == PB2_MAT_SUBSTRATE) {
+    if ((F & SHADE_SPECULAR) && mat.type == PB2_MAT_SUBSTRATE) {
         // substrate.cpp:45-65
         V3 d = clampSpectrum(mat.kd), sp = clampSpectrum(mat.ks);
         if (!isBlack(d) || !isBlack(sp)) {
@@ -469,7 +474,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         }
         return true;
     }
-    if (SPEC && mat.type == PB2_MAT_MIRROR) {
+    if ((F & SHADE_SPECULAR) && mat.type == PB2_MAT_MIRROR) {
         // mirror.cpp:45-58
         V3 r = clampSpectrum(mat.kr);
         if (!isBlack(r)) {
@@ -478,7 +483,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         }
         return true;
     }
-    if (SPEC && mat.type == PB2_MAT_GLASS && !(mat.uroughness == 0 && mat.vroughness == 0)) {
+    if ((F & SHADE_SPECULAR) && mat.type == PB2_MAT_GLASS && !(mat.uroughness == 0 && mat.vroughness == 0)) {
         // glass.cpp:45-93, rough: MicrofacetReflection(R, distrib, FresnelDielectric(1, eta)) + MicrofacetTransmission(T, distrib, 1, eta)
         V3 r = clampSpectrum(mat.kr), t = clampSpectrum(mat.kt);
         bsdf->eta = mat.eta;
@@ -503,7 +508,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         }
         return true;
     }
-    if (SPEC && mat.type == PB2_MAT_GLASS) {
+    if ((F & SHADE_SPECULAR) && mat.type == PB2_MAT_GLASS) {
         // glass.cpp:45-68 with urough == vrough == 0 and allowMultipleLobes (path.cpp:106): one FresnelSpecular
         V3 r = clampSpectrum(mat.kr), t = clampSpectrum(mat.kt);
         bsdf->eta = mat.eta;
@@ -519,7 +524,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
         float sig = clampf(mat.sigma, 0.f, 90.f);
         if (!isBlack(kd)) {
             bsdf->R = kd;
-            if (!(FC & SHADE_OREN_NAYAR) || sig == 0)
+            if (!(F & SHADE_OREN_NAYAR) || sig == 0)
                 bsdf->diffuseKind = 1;
             else {
                 bsdf->diffuseKind = 2;
@@ -537,7 +542,7 @@ PB2_HD bool makeBsdf(const DScene &sc, const DInteraction &it, DBsdf *bsdf, cons
             bsdf->nLobes++;
         }
         V3 ks = clampSpectrum(mat.ks);
-        if ((FC & SHADE_MICROFACET) && !isBlack(ks)) {
+        if ((F & SHADE_MICROFACET) && !isBlack(ks)) {
             float rough = mat.roughness;
             if (mat.remap_roughness) rough = roughnessToAlpha(rough);
             bsdf->Ks = ks;
@@ -714,9 +719,9 @@ PB2_HD float blendPdf(const DBsdf &b, V3 wo, V3 wi) {
 }
 
 // individual BxDFs (local frame)
-template <int FC = SHADE_ALL>
+template <int F>
 PB2_HD V3 diffuseF(const DBsdf &b, V3 wo, V3 wi) {
-    if (!(FC & SHADE_OREN_NAYAR) || b.diffuseKind == 1) return b.R * kInvPi;
+    if (!(F & SHADE_OREN_NAYAR) || b.diffuseKind == 1) return b.R * kInvPi;
     // OrenNayar::f (reflection.cpp:197-219)
     float sinThetaI = sinTheta(wi), sinThetaO = sinTheta(wo);
     float maxCos = 0;
@@ -844,28 +849,28 @@ PB2_HD V3 genF(const DBsdf &b, V3 wo, V3 wi, bool reflect) {
 
 // BSDF::f (reflection.cpp:680-693).  All lobes in scope are reflective and non-specular, so they
 // match both BSDF_ALL and BSDF_ALL & ~BSDF_SPECULAR.
-template <bool SPEC = true, int FC = SHADE_ALL>
+template <int F>
 PB2_HD V3 bsdfF(const DBsdf &b, V3 woW, V3 wiW) {
     V3 wi = worldToLocal(b, wiW), wo = worldToLocal(b, woW);
     if (wo.z == 0) return mk3(0, 0, 0);
     bool reflect = dot(wiW, b.ng) * dot(woW, b.ng) > 0;
     V3 f = mk3(0, 0, 0);
-    if (SPEC && b.blend) return reflect ? blendF(b, wo, wi) : f;
-    if (SPEC && b.general) return genF(b, wo, wi, reflect);
+    if ((F & SHADE_SPECULAR) && b.blend) return reflect ? blendF(b, wo, wi) : f;
+    if ((F & SHADE_SPECULAR) && b.general) return genF(b, wo, wi, reflect);
     if (reflect) {
-        if (b.diffuseKind) f = f + diffuseF<FC>(b, wo, wi);
-        if ((FC & SHADE_MICROFACET) && b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
+        if (b.diffuseKind) f = f + diffuseF<F>(b, wo, wi);
+        if ((F & SHADE_MICROFACET) && b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
     }
     return f;
 }
 // BSDF::Pdf (reflection.cpp:781-796)
-template <bool SPEC = true, int FC = SHADE_ALL>
+template <int F>
 PB2_HD float bsdfPdf(const DBsdf &b, V3 woW, V3 wiW) {
     if (b.nLobes == 0) return 0.f;
     V3 wo = worldToLocal(b, woW), wi = worldToLocal(b, wiW);
     if (wo.z == 0) return 0.;
-    if (SPEC && b.blend) return blendPdf(b, wo, wi);
-    if (SPEC && b.general) {
+    if ((F & SHADE_SPECULAR) && b.blend) return blendPdf(b, wo, wi);
+    if ((F & SHADE_SPECULAR) && b.general) {
         // the callers ask with BSDF_ALL & ~BSDF_SPECULAR (integrator.cpp:134): matchingComps == nLobes
         float pdf = 0.f;
         if (b.general & GEN_LAMBERT) pdf += diffusePdf(wo, wi);
@@ -875,7 +880,7 @@ PB2_HD float bsdfPdf(const DBsdf &b, V3 woW, V3 wiW) {
     }
     float pdf = 0.f;
     if (b.diffuseKind) pdf += diffusePdf(wo, wi);
-    if ((FC & SHADE_MICROFACET) && b.hasMicrofacet) pdf += microfacetPdf(b, wo, wi);
+    if ((F & SHADE_MICROFACET) && b.hasMicrofacet) pdf += microfacetPdf(b, wo, wi);
     return pdf / b.nLobes;
 }
 // BSDF::Sample_f (reflection.cpp:714-779).  Returns f; *pdf == 0 means no sample.
@@ -975,12 +980,12 @@ PB2_HDN V3 genSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
 }
 
 // *sampledFlags (optional): BSDF_SAMPLED_* of the BxDF that was sampled.
-template <bool SPEC = true, int FC = SHADE_ALL>
+template <int F>
 PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sampledFlags = nullptr, bool nonSpecularOnly = false) {
     *pdf = 0;
     if (sampledFlags) *sampledFlags = 0;
-    if (SPEC && b.general) return genSampleF(b, woW, wiW, u, pdf, sampledFlags, nonSpecularOnly);
-    if (SPEC && b.specKind) {
+    if ((F & SHADE_SPECULAR) && b.general) return genSampleF(b, woW, wiW, u, pdf, sampledFlags, nonSpecularOnly);
+    if ((F & SHADE_SPECULAR) && b.specKind) {
         // the BSDF holds exactly one BxDF, a specular one: matchingComps == 1, u is handed through
         // (uRemapped[0] = min(u[0], OneMinusEpsilon)), no pdf averaging and no re-evaluation of f
         // (reflection.cpp:725-775)
@@ -996,11 +1001,11 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
         } else {
             // FresnelSpecular::Sample_f (reflection.cpp:487-521), etaA = 1, etaB = eta, TransportMode::Radiance
             float u0 = pmin(u.x, kOneMinusEpsilon);
-            float F = frDielectric(cosTheta(wo), 1.f, b.eta);
-            if (u0 < F) {
+            float Fr = frDielectric(cosTheta(wo), 1.f, b.eta);
+            if (u0 < Fr) {
                 wi = mk3(-wo.x, -wo.y, wo.z);
-                *pdf = F;
-                V3 fr = F * b.specR;
+                *pdf = Fr;
+                V3 fr = Fr * b.specR;
                 f = mk3(fr.x / absCosTheta(wi), fr.y / absCosTheta(wi), fr.z / absCosTheta(wi));
             } else {
                 bool entering = cosTheta(wo) > 0;
@@ -1009,10 +1014,10 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
                 V3 nn = mk3(0, 0, 1);
                 if (dot(nn, wo) < 0) nn = -nn;  // Faceforward
                 if (!refract(wo, nn, etaI / etaT, &wi)) return mk3(0, 0, 0);
-                V3 ft = b.specT * (1 - F);
+                V3 ft = b.specT * (1 - Fr);
                 ft = ft * ((etaI * etaI) / (etaT * etaT));
                 flags |= BSDF_SAMPLED_TRANSMISSION;
-                *pdf = 1 - F;
+                *pdf = 1 - Fr;
                 f = mk3(ft.x / absCosTheta(wi), ft.y / absCosTheta(wi), ft.z / absCosTheta(wi));
             }
         }
@@ -1023,7 +1028,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     }
     int matching = b.nLobes;
     if (matching == 0) return mk3(0, 0, 0);
-    if (SPEC && b.blend) {
+    if ((F & SHADE_SPECULAR) && b.blend) {
         // one glossy BxDF: comp 0, uRemapped[0] = min(u[0], OneMinusEpsilon); FresnelBlend::Sample_f
         // (reflection.cpp:460-478); f is then re-evaluated by the BSDF (reflection.cpp:767-775)
         V3 wo = worldToLocal(b, woW), wi;
@@ -1048,7 +1053,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     int comp = (int)floorf(u.x * matching);
     if (comp > matching - 1) comp = matching - 1;
     // lobe order: diffuse first, then microfacet (plastic.cpp:53-68)
-    bool sampleMicro = (FC & SHADE_MICROFACET) && b.hasMicrofacet && (comp == matching - 1) && !(b.diffuseKind && comp == 0);
+    bool sampleMicro = (F & SHADE_MICROFACET) && b.hasMicrofacet && (comp == matching - 1) && !(b.diffuseKind && comp == 0);
     V2 uRemapped = mk2(pmin(u.x * matching - comp, kOneMinusEpsilon), u.y);
     V3 wo = worldToLocal(b, woW), wi;
     if (wo.z == 0) return mk3(0, 0, 0);
@@ -1058,7 +1063,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
         wi = cosineSampleHemisphere(uRemapped);
         if (wo.z < 0) wi.z *= -1;
         *pdf = diffusePdf(wo, wi);
-        f = diffuseF<FC>(b, wo, wi);
+        f = diffuseF<F>(b, wo, wi);
     } else {
         // MicrofacetReflection::Sample_f (reflection.cpp:410-423); wo.z == 0 handled above
         V3 wh = trSampleWh(b.alpha, wo, uRemapped);
@@ -1070,7 +1075,7 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     }
     if (*pdf == 0) return mk3(0, 0, 0);
     *wiW = localToWorld(b, wi);
-    if ((FC & SHADE_MICROFACET) && matching > 1) {   // (two lobes: plastic's)
+    if ((F & SHADE_MICROFACET) && matching > 1) {   // (two lobes: plastic's)
         if (sampleMicro) *pdf += diffusePdf(wo, wi);
         else *pdf += microfacetPdf(b, wo, wi);
         *pdf /= matching;
@@ -1079,8 +1084,8 @@ PB2_HD V3 bsdfSampleF(const DBsdf &b, V3 woW, V3 *wiW, V2 u, float *pdf, int *sa
     bool reflect = dot(*wiW, b.ng) * dot(woW, b.ng) > 0;
     f = mk3(0, 0, 0);
     if (reflect) {
-        if (b.diffuseKind) f = f + diffuseF<FC>(b, wo, wi);
-        if ((FC & SHADE_MICROFACET) && b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
+        if (b.diffuseKind) f = f + diffuseF<F>(b, wo, wi);
+        if ((F & SHADE_MICROFACET) && b.hasMicrofacet) f = f + microfacetF(b, wo, wi);
     }
     return f;
 }
@@ -1386,13 +1391,13 @@ PB2_HDN float infinitePdfLi(const DDeltaLight &dl, V3 w) {
 }
 
 // `rec` is the light's record out of DScene::lightRecs, lightNum its index in Scene::lights.
-template <bool SPH = true, int FC = SHADE_ALL>
+template <int F>
 PB2_HD DLightSample sampleLight(const DScene &sc, int lightNum, const pb2_light &l, const TriRec &rec, const DInteraction &ref, V2 u) {
-    const bool nonArea = (FC & SHADE_NON_AREA) && sc.deltaLights;
+    const bool nonArea = (F & SHADE_NON_AREA) && sc.deltaLights;
     if (nonArea && l.type == PB2_LIGHT_INFINITE) return sampleInfiniteLight(sc, l, sc.deltaLights[lightNum], ref.p, u);
     if (nonArea && l.type != PB2_LIGHT_AREA) return sampleDeltaLight(l, sc.deltaLights[lightNum], ref.p);
     DLightSample s;
-    if (SPH && (rec.flags & LEAF_SPHERE)) s = sampleSphereLight(sc, l, ref, u);
+    if ((F & SHADE_SPHERES) && (rec.flags & LEAF_SPHERE)) s = sampleSphereLight(sc, l, ref, u);
     else s = sampleTriangleLight(sc, l, rec, ref.p, u);
     s.delta = false;
     return s;
@@ -1400,10 +1405,10 @@ PB2_HD DLightSample sampleLight(const DScene &sc, int lightNum, const pb2_light 
 
 // DiffuseAreaLight::Pdf_Li -> Shape::Pdf(ref, wi) (shape.cpp:78-95): re-intersect the light's own
 // shape with the spawned ray and convert the area density to solid angle.
-template <bool SPH = true, int FC = SHADE_ALL>
+template <int F>
 PB2_HD float lightPdfLi(const DScene &sc, const pb2_light &l, const TriRec &rec, const DInteraction &ref, V3 wi, int lightNum = -1) {
-    if ((FC & SHADE_NON_AREA) && sc.deltaLights && l.type == PB2_LIGHT_INFINITE) return infinitePdfLi(sc.deltaLights[lightNum], wi);
-    if (SPH && (rec.flags & LEAF_SPHERE)) return sphereLightPdf(sc, l, ref, wi);
+    if ((F & SHADE_NON_AREA) && sc.deltaLights && l.type == PB2_LIGHT_INFINITE) return infinitePdfLi(sc.deltaLights[lightNum], wi);
+    if ((F & SHADE_SPHERES) && (rec.flags & LEAF_SPHERE)) return sphereLightPdf(sc, l, ref, wi);
     DRay ray = spawnRay(ref, wi);
     const TriVerts t = rec.tv;
     DRaySetup rs = setupRay(ray.o, ray.d);
@@ -1478,7 +1483,7 @@ PB2_HD float voxelLightContribution(const DScene &sc, const DHalton &h, const DV
         intr.uv = mk2(0, 0);
         intr.prim = -1;
         V2 u = mk2(radicalInverse(h, 3, i), radicalInverse(h, 4, i));
-        DLightSample ls = sampleLight(sc, j, light, rec, intr, u);
+        DLightSample ls = sampleLight<SHADE_GENERAL | SHADE_SPHERES>(sc, j, light, rec, intr, u);
         if (ls.pdf > 0) contrib += luminance(ls.Li) / ls.pdf;
     }
     return contrib;

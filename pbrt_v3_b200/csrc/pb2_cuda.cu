@@ -400,8 +400,7 @@ struct pb2_scene {
     int nLights = 0;
     int bvhDepth = 0;  // maximum number of simultaneously pending far children = tree depth (scene BVH)
     int instDepth = 0; // the same for the deepest instanced object's BVH
-    bool hasSpecular = false;  // a mirror / glass material exists: the shade kernel with the specular BxDFs is used
-    int shadeClass = SHADE_ALL;   // shadeFeatureClass: SHADE_LAMBERT_AREA selects the shade step compiled for that class
+    int shadeFeatures = SHADE_GENERAL;   // recordShadeFeatures: the lobes, lights and specular materials of the records
     int devIndex = 0;             // entry of g_devs this copy lives on
     std::vector<pb2_scene *> replicas;   // primary only: the copies on g_devs[1..] (pb2_init_devices with several devices)
     bool lazyLightDist = false;   // spatial light distribution built on demand (DLightDist::slots)
@@ -505,7 +504,7 @@ __global__ void k_intersect(DScene sc, const pb2_ray *rays, int64_t n, pb2_hit *
     out.prim = -1;
     out.t = tMax;
     if (found) {
-        DInteraction it = hitInteraction<true>(sc, h, r, tMax);
+        DInteraction it = hitInteraction<SHADE_SPHERES>(sc, h, r, tMax);
         out.prim = it.prim;
         out.b[0] = h.b0; out.b[1] = h.b1; out.b[2] = h.b2;
         out.p[0] = it.p.x; out.p[1] = it.p.y; out.p[2] = it.p.z;
@@ -658,7 +657,7 @@ __global__ void k_li_samples(DScene sc, DRenderParams rp, const int32_t *pixelXY
         tc.cam = &rp.cam;
         tc.pFilm = pFilm;
         tc.diffScale = rp.diffScale;
-        laneAdvance<true, true, true>(sc, rp.halton, rp.path, ln, found, hit, tMax, &tc);
+        laneAdvance<SHADE_FULL>(sc, rp.halton, rp.path, ln, found, hit, tMax, &tc);
         if (ln.state == LS_DEFER) {   // lazy light distribution: the voxel has been requested; the host builds it and runs the sample again
             atomicAdd(deferred, 1);
             return;
@@ -916,7 +915,8 @@ struct TraceLaunch {
 };
 
 // allowChain: the caller is a render (the contexts are whole paths); pb2_trace_wavefront's contexts are bare rays.
-static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool allowChain = false) {
+// steps: the render's other kernels, for the PB2_VERBOSE line.
+static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool allowChain = false, const char *steps = "") {
     TraceLaunch t;
     const bool wantChain = allowChain && (flags & PB2_FLAG_CHAIN) != 0;
     const bool spheres = scene->d.spheres != nullptr;
@@ -1001,8 +1001,8 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
     CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
     static const int verbose = envInt("PB2_VERBOSE", 0);
     if (verbose)
-        fprintf(stderr, "pb2: trace kernel %s: %d regs, %zu B smem, %d blocks/SM, carve-out %d %%, BVH depth %d\n", t.name, fa.numRegs,
-                fa.sharedSizeBytes + t.smem, blocksPerSM, pct, scene->bvhDepth);
+        fprintf(stderr, "pb2: trace kernel %s: %d regs, %zu B smem, %d blocks/SM, carve-out %d %%, BVH depth %d%s\n", t.name, fa.numRegs,
+                fa.sharedSizeBytes + t.smem, blocksPerSM, pct, scene->bvhDepth, steps);
     t.grid = g_numSMs * blocksPerSM;
     *out = t;
     return PB2_OK;
@@ -1040,6 +1040,41 @@ static WfPool poolOf(const pb2_scene *scene, int capacity, int pipe = 0, int nPi
 // Resident blocks per SM of the SHADE_LAMBERT_AREA shade step (__launch_bounds__ minimum; DESIGN.md section 3)
 constexpr int kShadeLambertAreaMinBlocks = 4;
 
+typedef void (*GenKernel)(const DRenderParams *, WfPool, int, int);
+typedef void (*FinishKernel)(const DScene *, const DRenderParams *, WfPool, int, unsigned, float4 *);
+
+// One instantiation of a wavefront step's kernel and the shade features (SHADE_*) it is compiled for.
+template <typename K>
+struct StepKernel {
+    int features;
+    K fn;
+};
+template <bool SHADE, int MINB, int F>
+static StepKernel<AdvanceKernel> advanceStep() { return {F, k_wf_advance<SHADE, MINB, F>}; }
+
+// The instantiation compiled for the fewest features that contain the frame's, counting only the features the step reads:
+// those of its widest instantiation, which every table holds.
+template <typename K, size_t N>
+static const StepKernel<K> &stepKernel(const StepKernel<K> (&table)[N], int frame) {
+    int reads = 0;
+    for (const StepKernel<K> &k : table) reads |= k.features;
+    const StepKernel<K> *best = nullptr;
+    for (const StepKernel<K> &k : table)
+        if (!(frame & reads & ~k.features) && (!best || __builtin_popcount(k.features) < __builtin_popcount(best->features))) best = &k;
+    return *best;
+}
+
+// The shade features of a frame (SHADE_* in device/pb2_shade.cuh): those of the scene's material and light records
+// (recordShadeFeatures), and its spheres, its lazy light distribution, its image textures and the frame's sampler.
+static int frameShadeFeatures(const pb2_scene *scene, const DRenderParams &rp) {
+    int f = scene->shadeFeatures;
+    if (scene->d.spheres) f |= SHADE_SPHERES;
+    if (scene->lazyLightDist) f |= SHADE_LAZY;
+    if (scene->d.nTextures > 0) f |= SHADE_TEXTURES;
+    if (rp.halton.sobol) f |= SHADE_SOBOL;
+    return f;
+}
+
 // Host driver of the wavefront rounds (see pb2_wavefront.cuh).
 static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *film, cudaStream_t stream, int flags,
                            bool timeTrace, unsigned long long *launches, double *traceMs) {
@@ -1050,8 +1085,45 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     int capacity = (int)((want + 255) / 256 * 256);
     int rc = ensurePool(scene, capacity);
     if (rc) return rc;
+    // Each step runs the kernel compiled for the frame's shade features (stepKernel): Lambertian surfaces lit by area lights
+    // (the bench scene) get the class-0 kernels.
+    static const StepKernel<GenKernel> genSteps[] = {{0, k_wf_gen<0>}, {SHADE_SOBOL, k_wf_gen<SHADE_SOBOL>}};
+    // light step: 7 resident blocks, as many as the shared-memory stage leaves room for (29 KB per block)
+    static const StepKernel<AdvanceKernel> lightSteps[] = {
+        advanceStep<false, 7, SHADE_LAMBERT_AREA>(),
+        advanceStep<false, 7, SHADE_GENERAL>(),
+        advanceStep<false, 7, SHADE_GENERAL | SHADE_SPHERES>(),
+    };
+    // image textures or the SobolSampler: one shade kernel with everything compiled in (3 resident blocks, its register
+    // budget is not the bench scene's)
+    static const StepKernel<AdvanceKernel> shadeSteps[] = {
+        advanceStep<true, kShadeLambertAreaMinBlocks, SHADE_LAMBERT_AREA>(),
+        advanceStep<true, 4, SHADE_GENERAL>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_SPHERES>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_SPECULAR>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_SPHERES | SHADE_SPECULAR>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_LAZY>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_SPHERES | SHADE_LAZY>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_SPECULAR | SHADE_LAZY>(),
+        advanceStep<true, 4, SHADE_GENERAL | SHADE_SPHERES | SHADE_SPECULAR | SHADE_LAZY>(),
+        advanceStep<true, 3, SHADE_FULL>(),
+    };
+    static const StepKernel<FinishKernel> finishSteps[] = {
+        {SHADE_LAMBERT_AREA, k_wf_finish<SHADE_LAMBERT_AREA>},
+        {SHADE_GENERAL, k_wf_finish<SHADE_GENERAL>},
+        {SHADE_GENERAL | SHADE_SPHERES, k_wf_finish<SHADE_GENERAL | SHADE_SPHERES>},
+        {SHADE_GENERAL | SHADE_SPECULAR, k_wf_finish<SHADE_GENERAL | SHADE_SPECULAR>},
+        {SHADE_GENERAL | SHADE_SPHERES | SHADE_SPECULAR, k_wf_finish<SHADE_GENERAL | SHADE_SPHERES | SHADE_SPECULAR>},
+    };
+    const int features = frameShadeFeatures(scene, rp);
+    const StepKernel<GenKernel> &gen = stepKernel(genSteps, features);
+    const StepKernel<AdvanceKernel> &advLight = stepKernel(lightSteps, features), &advShade = stepKernel(shadeSteps, features);
+    const StepKernel<FinishKernel> &finish = stepKernel(finishSteps, features);
+    char steps[96];
+    snprintf(steps, sizeof(steps), "; shade features %d: gen %d, light %d, shade %d, tail %d", features, gen.features,
+             advLight.features, advShade.features, finish.features);
     TraceLaunch trace;
-    if ((rc = selectTraceKernel(scene, flags, &trace, true))) return rc;
+    if ((rc = selectTraceKernel(scene, flags, &trace, true, steps))) return rc;
     // the scene and this frame's parameters as objects in device memory, read by the gen / advance / finish kernels and
     // wfChainLight.  One buffer per scene, and so per device: every device of a group renders its own replica.
     if (!scene->paramBuf) CUDA_TRY(cudaMalloc(&scene->paramBuf, sizeof(DScene) + sizeof(DRenderParams)));
@@ -1066,36 +1138,10 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         chain.rp = dRp;
         chain.film = film;
     }
-    const bool spheres = scene->d.spheres != nullptr;
-    // Lambertian surfaces lit by area lights (the bench scene): the shade step, the light step and the tail compiled for that
-    // class alone (device/pb2_shade.cuh, SHADE_*).  Scenes with spheres, the lazy light distribution, image textures or the
-    // SobolSampler keep the general instantiations.
-    const bool sobol = rp.halton.sobol != nullptr;
-    const bool textured = scene->d.nTextures > 0 || sobol;
-    const bool lambertArea = scene->shadeClass == SHADE_LAMBERT_AREA && !scene->hasSpecular && !spheres;
-    const bool narrowShade = lambertArea && !scene->lazyLightDist && !textured;
-    // light step: 7 resident blocks, as many as the shared-memory stage leaves room for (29 KB per block)
-    AdvanceKernel advLight = spheres ? k_wf_advance<false, true, 7> : k_wf_advance<false, false, 7>;
-    if (lambertArea) advLight = k_wf_advance<false, false, 7, false, false, false, SHADE_LAMBERT_AREA>;
-    AdvanceKernel advShade = scene->hasSpecular ? (spheres ? k_wf_advance<true, true, 4, true> : k_wf_advance<true, false, 4, true>)
-                             : spheres ? k_wf_advance<true, true, 4>
-                                       : k_wf_advance<true, false, 4>;
-    if (scene->lazyLightDist)   // the shade kernels that can hand a vertex back (DLightDist::slots)
-        advShade = scene->hasSpecular ? (spheres ? k_wf_advance<true, true, 4, true, true> : k_wf_advance<true, false, 4, true, true>)
-                   : spheres ? k_wf_advance<true, true, 4, false, true>
-                             : k_wf_advance<true, false, 4, false, true>;
-    // image textures: the one shade kernel that evaluates them (spheres, specular materials and the lazy light distribution
-    // compiled in; 3 resident blocks, its register budget is not the bench scene's)
-    // ... and the one that draws from the SobolSampler: the same general instantiation
-    if (textured) advShade = k_wf_advance<true, true, 3, true, true, true>;
-    if (narrowShade) advShade = k_wf_advance<true, false, kShadeLambertAreaMinBlocks, false, false, false, SHADE_LAMBERT_AREA>;
-    typedef void (*FinishKernel)(const DScene *, const DRenderParams *, WfPool, int, unsigned, float4 *);
-    FinishKernel finish = scene->hasSpecular ? (spheres ? k_wf_finish<true, true> : k_wf_finish<false, true>)
-                                             : (spheres ? k_wf_finish<true, false> : k_wf_finish<false, false>);
-    if (lambertArea) finish = k_wf_finish<false, false, SHADE_LAMBERT_AREA>;
     // the frame's last paths are walked to their end by one thread each once this few are left (k_wf_finish)
     static const int finishPerSM = envInt("PB2_FINISH", 256);
-    // (textured scenes: the tail kernel's lane functions are the untextured instantiation, so the rounds run to the end)
+    // (image textures or the SobolSampler: the tail kernels are compiled without them, so the rounds run to the end)
+    const bool textured = (features & (SHADE_TEXTURES | SHADE_SOBOL)) != 0;
     const unsigned finishThreshold = ((flags & PB2_FLAG_COUNT_TRAVERSAL) || lazyLights || textured) ? 0u : (unsigned)(g_numSMs * std::max(0, finishPerSM));
     const int finishBlocks = std::max(1, (int)((finishThreshold + 127) / 128));
     static const int syncEvery = std::max(1, envInt("PB2_SYNC_EVERY", 8));
@@ -1135,8 +1181,7 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
         for (int p = 0; p < nPipes; ++p) {
             const WfPool &pool = pools[p];
             cudaStream_t st = streams[p];
-            if (sobol) k_wf_gen<true><<<blocks128, 128, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
-            else k_wf_gen<false><<<blocks128, 128, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
+            gen.fn<<<blocks128, 128, 0, st>>>(dRp, pool, WQ_FREE0 + cur, WQ_TRACE0 + cur);
             if (timeTrace) {
                 if (scene->traceEvents.size() < nEvents + 2) {
                     cudaEvent_t e0, e1;
@@ -1153,16 +1198,16 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
                 CUDA_TRY(cudaEventRecord(scene->traceEvents[nEvents + 1], st));
                 nEvents += 2;
             }
-            if (!trace.chain) advLight<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_LIGHT, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
+            if (!trace.chain) advLight.fn<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_LIGHT, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
             else --nLaunch;
-            advShade<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_SHADE, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
+            advShade.fn<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_SHADE, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
             if (lazyLights) {
                 // vertices that fell into voxels without a light distribution yet were put aside: build those records, shade again
                 launchLightDistBuild(scene, st);
-                advShade<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_RETRY, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
+                advShade.fn<<<blocks128, 128, 0, st>>>(dSc, dRp, pool, WQ_RETRY, WQ_TRACE0 + next, WQ_FREE0 + next, film, scene->counters);
                 nLaunch += 3;
             }
-            if (finishThreshold) finish<<<finishBlocks, 128, 0, st>>>(dSc, dRp, pool, WQ_TRACE0 + next, finishThreshold, film);
+            if (finishThreshold) finish.fn<<<finishBlocks, 128, 0, st>>>(dSc, dRp, pool, WQ_TRACE0 + next, finishThreshold, film);
             k_wf_reset<<<1, 32, 0, st>>>(pool, WQ_FREE0 + cur, WQ_TRACE0 + cur, WQ_TRACE0 + next, finishThreshold);
             nLaunch += finishThreshold ? 6 : 5;
         }
@@ -1518,12 +1563,12 @@ int pb2_scene_create(const pb2_scene_desc *d, pb2_scene **out) {
     return PB2_OK;
 }
 
-static int shadeFeatureClass(const pb2_scene_desc *d);
+static int recordShadeFeatures(const pb2_scene_desc *d);
 int pb2_shade_class(const pb2_scene_desc *d, int32_t *out) {
     if (!d || !out) return setError(PB2_ERR_INVALID, "null argument");
     if (d->n_materials < 0 || (d->n_materials > 0 && !d->materials) || d->n_lights < 0 || (d->n_lights > 0 && !d->lights))
         return setError(PB2_ERR_INVALID, "bad material or light records");
-    *out = shadeFeatureClass(d);
+    *out = recordShadeFeatures(d) & SHADE_GENERAL;
     return PB2_OK;
 }
 
@@ -1841,13 +1886,12 @@ extern "C" int pb2_env_distribution(const pb2_texture *texture, int32_t *nu, int
     return PB2_OK;
 }
 
-// The scene's shade feature class (SHADE_* in device/pb2_shade.cuh): a bit stays clear only when no record of the scene
-// can take the branch it stands for, so the class's kernels compute what the general ones do.  PB2_SHADE_GENERAL=1 gives
-// every scene the general class (tests compare the two).
-static int shadeFeatureClass(const pb2_scene_desc *d) {
+// The shade features of the scene's material and light records (SHADE_* in device/pb2_shade.cuh): a bit stays clear only
+// when no record of the scene can take the branch it stands for, so kernels compiled without it compute what the general
+// ones do.  PB2_SHADE_GENERAL=1 gives every scene the general class (tests compare the two).
+static int recordShadeFeatures(const pb2_scene_desc *d) {
     static const bool forceGeneral = envInt("PB2_SHADE_GENERAL", 0) != 0;
-    if (forceGeneral) return SHADE_ALL;
-    int fc = 0;
+    int fc = forceGeneral ? SHADE_GENERAL : 0;
     for (int i = 0; i < d->n_materials; ++i) {
         const pb2_material &m = d->materials[i];
         if (m.type == PB2_MAT_NONE) continue;
@@ -1857,7 +1901,7 @@ static int shadeFeatureClass(const pb2_scene_desc *d) {
         } else if (m.type == PB2_MAT_PLASTIC)
             fc |= SHADE_MICROFACET;
         else
-            return SHADE_ALL;   // the specular family: the SPEC kernels, which are compiled for every class
+            fc |= SHADE_SPECULAR | SHADE_GENERAL;   // the specular family: its kernels are compiled for the general class
     }
     for (int i = 0; i < d->n_lights; ++i)
         if (d->lights[i].type != PB2_LIGHT_AREA) fc |= SHADE_NON_AREA;
@@ -1897,11 +1941,7 @@ static int createSceneOnCurrentDevice(const pb2_scene_desc *d, pb2_scene **out) 
     } guard{new pb2_scene()};
     pb2_scene *s = guard.s;
     s->devIndex = t_dev;
-    for (int i = 0; i < d->n_materials; ++i)
-        if (d->materials[i].type == PB2_MAT_MIRROR || d->materials[i].type == PB2_MAT_GLASS || d->materials[i].type == PB2_MAT_SUBSTRATE ||
-            d->materials[i].type == PB2_MAT_METAL || d->materials[i].type == PB2_MAT_UBER)
-            s->hasSpecular = true;
-    s->shadeClass = shadeFeatureClass(d);
+    s->shadeFeatures = recordShadeFeatures(d);
     DScene &sc = s->d;
     memset(&sc, 0, sizeof(sc));
     sc.nNodes = d->n_nodes;
@@ -2719,15 +2759,17 @@ int pb2_bsdf_eval_host(const pb2_material *material, int64_t n, const float *in,
         const V3 wo = mk3(q[9], q[10], q[11]), wi = mk3(q[12], q[13], q[14]);
         it.wo = wo;
         it.prim = 0;
+        // every lobe of every material; the texture slots are not evaluated
+        constexpr int F = SHADE_GENERAL | SHADE_SPECULAR;
         DBsdf bsdf;
-        if (!makeBsdf<true>(sc, it, &bsdf)) continue;
+        if (!makeBsdf<F>(sc, it, &bsdf)) continue;
         if (bsdf.nLobes > 0) {   // (EstimateDirect is only entered with non-specular lobes: path.cpp:119-126)
-            const V3 f = bsdfF<true>(bsdf, wo, wi);
+            const V3 f = bsdfF<F>(bsdf, wo, wi);
             o[0] = f.x; o[1] = f.y; o[2] = f.z;
-            o[3] = bsdfPdf<true>(bsdf, wo, wi);
+            o[3] = bsdfPdf<F>(bsdf, wo, wi);
             V3 wiS;
             float pdfS;
-            const V3 fS = bsdfSampleF<true>(bsdf, wo, &wiS, mk2(q[15], q[16]), &pdfS, nullptr, true);
+            const V3 fS = bsdfSampleF<F>(bsdf, wo, &wiS, mk2(q[15], q[16]), &pdfS, nullptr, true);
             if (pdfS != 0) { o[4] = wiS.x; o[5] = wiS.y; o[6] = wiS.z; }
             o[7] = fS.x; o[8] = fS.y; o[9] = fS.z;
             o[10] = pdfS;
@@ -2735,7 +2777,7 @@ int pb2_bsdf_eval_host(const pb2_material *material, int64_t n, const float *in,
         V3 wiC;
         float pdfC;
         int flags = 0;
-        const V3 fC = bsdfSampleF<true>(bsdf, wo, &wiC, mk2(q[15], q[16]), &pdfC, &flags);
+        const V3 fC = bsdfSampleF<F>(bsdf, wo, &wiC, mk2(q[15], q[16]), &pdfC, &flags);
         if (pdfC != 0) { o[11] = wiC.x; o[12] = wiC.y; o[13] = wiC.z; }
         o[14] = fC.x; o[15] = fC.y; o[16] = fC.z;
         o[17] = pdfC;

@@ -234,7 +234,7 @@ struct WfChain {
 // The hit is the one the trace kernel has just stored in the context ((leaf, b0, b1, b2), tHit, the found code), decoded
 // as k_wf_advance does: a MIS ray that reaches a one-sided area light is counted only when the light's surface at the
 // hit faces the ray, and a triangle's surface is built from the hit's barycentrics (its shading normals) and instance.
-template <bool SPH>
+template <int F>
 __device__ __noinline__ int wfChainLight(const WfChain &ch, WfCtx *cx, bool found) {
     DLane &ln = cx->ln;
     const float4 h4 = cx->hit;
@@ -245,7 +245,7 @@ __device__ __noinline__ int wfChainLight(const WfChain &ch, WfCtx *cx, bool foun
     hit.b1 = h4.z;
     hit.b2 = h4.w;
     hit.inst = foundCode >= 2 ? foundCode - 2 : -1;
-    lightAdvance<SPH>(*ch.sc, ln, found, hit, cx->tHit);
+    lightAdvance<F>(*ch.sc, ln, found, hit, cx->tHit);
     if (ln.state == LS_IDLE) addSample(*ch.rp, ch.film, cx->pFilm, guardRadiance(ln.L));
     return ln.state;
 }
@@ -290,11 +290,10 @@ __device__ __forceinline__ bool wfStartSample(const DRenderParams &rp, const WfP
 
 // Contexts on the free list take their next sample.  (Not inside k_wf_advance: there the few lanes of a warp that end a
 // path would run this code alone inside the register-heavy, low-occupancy shade kernel.)
-// GENERAL = true: the instantiation that can also draw from the SobolSampler (frames that use it).
 // The scene and the frame's parameters come as objects in device memory (renderWavefront uploads them once per render):
 // a struct passed by value whose address reaches a device function is copied to every thread's stack at kernel entry.
 // The new lanes are built in shared memory and written out as whole sectors (WF_OUT_START), pFilm as one 8-byte store.
-template <bool GENERAL>
+template <int F>
 __global__ void __launch_bounds__(128) k_wf_gen(const DRenderParams *__restrict__ rpp, WfPool pool, int freeQ, int traceQ) {
     __shared__ WfSlot stage[128];
     WfSlot &slot = stage[threadIdx.x];
@@ -309,7 +308,7 @@ __global__ void __launch_bounds__(128) k_wf_gen(const DRenderParams *__restrict_
         unsigned i = base + threadIdx.x;
         const bool have = i < n;
         const int c = have ? freeList[i] : -1;
-        const bool started = wfStartSample<GENERAL>(rp, pool, slot, have, &cameraRays);
+        const bool started = wfStartSample<(F & SHADE_SOBOL) != 0>(rp, pool, slot, have, &cameraRays);
         if (started) {
             slot.ln.lightNum = 0;   // (not read before the shade step sets them: written only to store no stale shared memory)
             slot.ln.pick = 0;
@@ -980,7 +979,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool
                 // continuation) in this lane, in this launch - one round per bounce instead of up to three
                 int next = LS_PATH;
                 if (flush && state != LS_PATH) {
-                    next = wfChainLight<SPHERES>(chain, &pool.ctx[c], (flags & F_FOUND) != 0);
+                    next = wfChainLight<SHADE_GENERAL | (SPHERES ? SHADE_SPHERES : 0)>(chain, &pool.ctx[c], (flags & F_FOUND) != 0);
                     again = next != LS_IDLE;
                 }
                 const unsigned mShadow = __ballot_sync(FULL, again && next == LS_SHADOW), mRegular = __ballot_sync(FULL, again && next != LS_SHADOW);
@@ -1273,11 +1272,10 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool p
 // laneAdvance for every context of one list.  SHADE = true: the shade list (path rays: the whole
 // vertex is evaluated); SHADE = false: the light list (shadow / MIS rays: a few adds and the next
 // ray).  Two instantiations so that the light kernel is small and the warps of each stay converged.
+// F: the shade features (SHADE_* in device/pb2_shade.cuh) the step is compiled for.  With SHADE_TEXTURES the camera ray's
+// differentials are rebuilt from the context's pFilm.
 // ---------------------------------------------------------------------------------------------
-// TEX = true: the shade step of a scene with image textures (the camera ray's differentials are rebuilt from the
-// context's pFilm); one instantiation, with everything else compiled in.
-// FC: the scene's shade feature class (SHADE_* in device/pb2_shade.cuh); SHADE_ALL is the general instantiation.
-template <bool SHADE, bool SPH, int MINB, bool SPEC = false, bool LAZY = false, bool TEX = false, int FC = SHADE_ALL>
+template <bool SHADE, int MINB, int F>
 __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool,
                                                           int srcQ, int traceQ, int freeQ, float4 *film, unsigned long long *counters) {
     __shared__ WfSlot stage[128];
@@ -1311,15 +1309,15 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
             hit.inst = foundCode >= 2 ? foundCode - 2 : -1;
             bool found = foundCode != 0;
             float tHit = slot.tHit;
-            if (SHADE && TEX) {
+            if (SHADE && (F & SHADE_TEXTURES)) {
                 DTexCtx tc;
                 tc.cam = &rp.cam;
                 tc.pFilm = slot.pFilm;
                 tc.diffScale = rp.diffScale;
-                shadeVertex<SPH, SPEC, LAZY, true>(sc, rp.halton, rp.path, ln, found, hit, tHit, u, &tc);
-            } else if (SHADE) shadeVertex<SPH, SPEC, LAZY, false, FC>(sc, rp.halton, rp.path, ln, found, hit, tHit, u);
-            else lightAdvance<SPH, FC>(sc, ln, found, hit, tHit);
-            if (SHADE && LAZY && ln.state == LS_DEFER) {
+                shadeVertex<F>(sc, rp.halton, rp.path, ln, found, hit, tHit, u, &tc);
+            } else if (SHADE) shadeVertex<F>(sc, rp.halton, rp.path, ln, found, hit, tHit, u);
+            else lightAdvance<F>(sc, ln, found, hit, tHit);
+            if (SHADE && (F & SHADE_LAZY) && ln.state == LS_DEFER) {
                 ln.state = LS_PATH;   // untouched: shaded again from the retry list once its voxel's record exists
                 deferred = true;
             } else {
@@ -1331,7 +1329,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
         }
         // (an ended path's lane is not written back: its context goes to the free list, and k_wf_gen starts a new lane in it)
         wfStageOut<SHADE ? WF_OUT_SHADE : WF_OUT_LIGHT>(pool.ctx, warpSlots, have && !ended ? c : -1);
-        if (SHADE && LAZY) wfPush(pool.queue[WQ_RETRY], &pool.counts[WQ_RETRY], c, deferred);
+        if (SHADE && (F & SHADE_LAZY)) wfPush(pool.queue[WQ_RETRY], &pool.counts[WQ_RETRY], c, deferred);
         wfPush(traceList, &pool.counts[traceQ], c, have && !ended && !deferred);
         wfPush(freeList, &pool.counts[freeQ], c, have && ended);
     }
@@ -1353,7 +1351,7 @@ __device__ __forceinline__ bool wfFinishNow(const DRenderParams &rp, const WfPoo
     return n > 0 && n <= threshold && (long long)pool.ctr[CTR_WORK] >= rp.nWorkItems;
 }
 
-template <bool SPH, bool SPEC, int FC = SHADE_ALL>
+template <int F>
 __global__ void __launch_bounds__(128) k_wf_finish(const DScene *__restrict__ scp, const DRenderParams *__restrict__ rpp, WfPool pool, int traceQ,
                                                    unsigned threshold, float4 *film) {
     const DScene &sc = *scp;
@@ -1380,7 +1378,7 @@ __global__ void __launch_bounds__(128) k_wf_finish(const DScene *__restrict__ sc
             DHit hit;
             float tMax;
             const bool found = traceLane(sc, ln, &tMax, &hit, nullptr);
-            laneAdvance<SPH, SPEC, false, FC>(sc, rp.halton, rp.path, ln, found, hit, tMax);
+            laneAdvance<F>(sc, rp.halton, rp.path, ln, found, hit, tMax);
             if (ln.state == LS_DEFER) break;            // (never: this kernel is not launched for lazily lit scenes)
             if (ln.state == LS_SHADOW) shadow++;        // the next ray is a Scene::IntersectP call
             else if (ln.state != LS_IDLE) regular++;    // ... a Scene::Intersect call
