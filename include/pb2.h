@@ -334,7 +334,7 @@ enum { PB2_SAMPLER_HALTON = 0, PB2_SAMPLER_SOBOL = 1 };
 /* Experiment kept for the record (DESIGN.md section 3): stage leaf records into shared memory with TMA bulk copies
  * (cp.async.bulk / UBLKCP + mbarrier) before the triangle tests; triangle scenes, two-child kernel.  Same results, slower. */
 #define PB2_FLAG_LEAF_TMA 64
-/* Trace triangle scenes with the kernel that keeps a pool of 64 rays per warp in shared memory and picks, for every step,
+/* Trace triangle scenes with the kernel that keeps a pool of 48 rays per warp in shared memory and picks, for every step,
  * the rays that are in the phase being run (k_wf_trace_pool).  Same results. */
 #define PB2_FLAG_POOL 128
 /* Experiment kept for the record (DESIGN.md section 3): the default trace kernels with the light step inside - when a shadow

@@ -1,4 +1,4 @@
-// Four-child node records: the layout the default trace kernel (k_wf_trace_w<4, ...>, pb2_wavefront.cuh) walks.
+// Four-child node records: the layout the four-child trace kernel (k_wf_trace_w<4, T>, pb2_wavefront.cuh) walks.
 //
 // One 128-B record per interior node of every second level of the reference's binary tree (src/accelerators/bvh.cpp:
 // 95-104, 640-658): the boxes of the node's grandchildren in the canonical slot order [LL, LR, RL, RR]; a child that is a

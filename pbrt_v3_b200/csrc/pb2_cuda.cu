@@ -893,102 +893,110 @@ enum { kMaxPipes = 4 };   // wavefront pipelines (renderWavefront)
 typedef void (*TraceKernel)(DScene, WfPool, int, WfChain);
 typedef void (*AdvanceKernel)(const DScene *, const DRenderParams *, WfPool, int, int, int, float4 *, unsigned long long *);
 
-// Which traversal kernel a scene is traced with (pb2_wavefront.cuh), and its launch shape.
-//   default                   k_wf_trace_w<2>: persistent warps over the two-child records (a record is read as
-//                             pairs of 16-byte loads, ldg256)
-//   PB2_FLAG_WIDE4            k_wf_trace_w<4>: the same over the four-child records (two tree levels per fetch)
-//   PB2_FLAG_LD128            either of them with one 16-byte load per quarter record (on sm_90 the same loads)
-//   PB2_FLAG_LINEAR_NODES     k_wf_trace: the same over the reference's 32-B LinearBVHNode array; also the fallback for
-//                             scenes beyond the record limits (2^27 primitives, 16 per leaf)
-//   PB2_FLAG_PLAIN_TRACE /    k_wf_trace_plain: one thread per ray, BVHAccel::Intersect as written (the counting form
-//   PB2_FLAG_COUNT_TRAVERSAL  also returns node / primitive counters)
-//   PB2_FLAG_SMALL_STACK      4 instead of 16 shared-memory stack entries per lane (tests: forces the local-memory spill)
-// The four-child visit needs as many instructions per box as the two-child one (ordering and up to three deferred
-// entries), so halving the dependent fetches need not pay; the two-child kernel is the default.
+// The launch shape of the trace kernel a scene is traced with.
 struct TraceLaunch {
     TraceKernel fn = nullptr;
     int block = 128;
     size_t smem = 0;
-    int grid = 0;          // persistent kernels: SMs x resident blocks; 0 = one thread per list entry (plain kernels)
+    int grid = 0;          // SMs x resident blocks: every trace kernel loops over its list
     bool chain = false;    // the kernel advances shadow / MIS rays itself (no k_wf_advance<light> launch)
     const char *name = "";
 };
 
-// allowChain: the caller is a render (the contexts are whole paths); pb2_trace_wavefront's contexts are bare rays.
-// steps: the render's other kernels, for the PB2_VERBOSE line.
-static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool allowChain = false, const char *steps = "") {
-    TraceLaunch t;
-    const bool wantChain = allowChain && (flags & PB2_FLAG_CHAIN) != 0;
-    const bool spheres = scene->d.spheres != nullptr;
+// The trace kernels (pb2_wavefront.cuh): k_wf_trace_plain, BVHAccel::Intersect as written (TK_COUNT: with node / primitive
+// counters), the ray-pool kernel, and the persistent warps over the two-child records (the default), the four-child records
+// and the reference's 32-B LinearBVHNode array (k_wf_trace).
+enum TraceKernelForm { TK_COUNT, TK_PLAIN, TK_POOL, TK_WIDE2, TK_WIDE4, TK_LINEAR };
+// One instantiation of a trace kernel and the trace features (TRACE_*) it is compiled for.
+struct TraceKernelEntry {
+    TraceKernelForm form;
+    int features;
+    TraceKernel fn;
+    const char *name;   // on the PB2_VERBOSE line
+    size_t smem;        // dynamic shared memory per block
+};
+template <int WIDTH, int T>
+static TraceKernelEntry wideTrace() {
+    const char *name = WIDTH == 4              ? "k_wf_trace_w<4>"
+                       : (T & TRACE_ALPHA) ? "k_wf_trace_w<2,alpha>"
+                       : (T & TRACE_CHAIN) ? "k_wf_trace_w<2,chain>"
+                                           : "k_wf_trace_w<2>";
+    return {WIDTH == 4 ? TK_WIDE4 : TK_WIDE2, T, k_wf_trace_w<WIDTH, T>, name, 0};
+}
+template <int T>
+static TraceKernelEntry linearTrace() { return {TK_LINEAR, T, k_wf_trace<T>, "k_wf_trace", 0}; }
+
+// The trace kernel for a scene and the PB2_FLAG_* of a call: its form and the features it must be compiled for.  The
+// first rule that matches wins, and a flag a rule does not name is ignored.  render: the caller is a render (the
+// contexts are whole paths); pb2_trace_wavefront's contexts are bare rays, which cannot be chained.
+struct TraceKey {
+    TraceKernelForm form;
+    int features;
+};
+static TraceKey chooseTraceKernel(const pb2_scene *scene, int flags, bool render) {
     const bool instanced = scene->d.instances != nullptr;
+    // the two- and four-child records exist for scenes within their limits (2^27 primitives, 16 per leaf)
     const bool records = scene->d.wide4 != nullptr && !(flags & PB2_FLAG_LINEAR_NODES);
-    const bool small = (flags & PB2_FLAG_SMALL_STACK) != 0;
     // the two levels of an instanced scene must fit the 64-entry stack of the 32-B-node kernel
     const bool linearFits = !instanced || scene->bvhDepth + 3 + scene->instDepth <= 64;
-    if (flags & PB2_FLAG_COUNT_TRAVERSAL) { t.fn = k_wf_trace_plain<true>; t.name = "k_wf_trace_plain<count>"; }
-    else if ((flags & PB2_FLAG_PLAIN_TRACE) || (!records && !linearFits)) { t.fn = k_wf_trace_plain<false>; t.name = "k_wf_trace_plain"; }
-    else if (scene->d.hasAlpha) {
-        // alpha-masked meshes: the default two-child kernel with the alpha test compiled in (the selector flags of the
-        // experiments are not honoured for such scenes); without records, the one-thread-per-ray traversal
-        if (!records) { t.fn = k_wf_trace_plain<false>; t.name = "k_wf_trace_plain"; }
-        else {
-            t.name = "k_wf_trace_w<2,alpha>";
-            if (instanced) t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 6, true, true, true, false, true>;
-            else if (spheres) t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 6, true, false, true, false, true>;
-            else t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 6, false, false, true, false, true>;
-        }
-    } else if (records && (flags & PB2_FLAG_POOL) && !spheres && !instanced) {
-        t.name = "k_wf_trace_pool";
-        if (!scene->wfSpill)   // per pipeline: up to 8 resident blocks per SM x 4 warps x PL_R slots x PL_SPILL entries
-            CUDA_TRY(cudaMalloc((void **)&scene->wfSpill, (size_t)kMaxPipes * g_numSMs * 8 * 4 * PL_R * PL_SPILL * sizeof(int2)));
-        // 48 rays per warp, 8 stack entries per ray in shared memory: 25 KB per block, 8 resident blocks per SM
-        t.fn = k_wf_trace_pool<4, 8, 16, 12, 48, 8>;
-        t.smem = 4 * sizeof(PoolWarp<48, 8>);
-        CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)t.smem));
-    } else if (records && (flags & PB2_FLAG_WIDE4)) {
-        t.name = "k_wf_trace_w<4>";
-        if (flags & PB2_FLAG_LD128) {
-            if (instanced) t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 5, true, true> : k_wf_trace_w<4, 1, 8, 4, 16, 5, true, true>;
-            else if (spheres) t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 5, true> : k_wf_trace_w<4, 1, 8, 4, 16, 5, true>;
-            else t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 7> : k_wf_trace_w<4, 1, 8, 4, 16, 7>;
-        } else {
-            if (instanced) t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 5, true, true, true> : k_wf_trace_w<4, 1, 8, 4, 16, 5, true, true, true>;
-            else if (spheres) t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 5, true, false, true> : k_wf_trace_w<4, 1, 8, 4, 16, 5, true, false, true>;
-            else t.fn = small ? k_wf_trace_w<4, 1, 8, 4, 4, 7, false, false, true> : k_wf_trace_w<4, 1, 8, 4, 16, 7, false, false, true>;
-        }
-    } else if (records) {
-        // LEAF_T = 1: a warp turns to its leaves as soon as one lane holds one; 56 registers (room for 9 blocks / SM)
-        t.name = "k_wf_trace_w<2>";
-        if (flags & PB2_FLAG_LD128) {
-            if (instanced) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true, true>;
-            else if (spheres) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true>;
-            else t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 9> : k_wf_trace_w<2, 1, 8, 4, 16, 9>;
-        } else {
-            if (instanced) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true, true, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true, true, true>;
-            else if (spheres) t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 6, true, false, true> : k_wf_trace_w<2, 1, 8, 4, 16, 6, true, false, true>;
-            else if (flags & PB2_FLAG_LEAF_TMA) t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 5, false, false, true, true>;
-            else t.fn = small ? k_wf_trace_w<2, 1, 8, 4, 4, 9, false, false, true> : k_wf_trace_w<2, 1, 8, 4, 16, 9, false, false, true>;
-            // (experiment, PB2_FLAG_CHAIN; not the default, DESIGN.md section 3) the default kernels with the light step
-            // inside: shadow ray -> MIS ray -> continuation follow each other in the lane, one round per bounce
-            if (wantChain && !small && !(flags & PB2_FLAG_LEAF_TMA)) {
-                t.chain = true;
-                t.name = "k_wf_trace_w<2,chain>";
-                if (instanced) t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 6, true, true, true, false, false, true>;
-                else if (spheres) t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 6, true, false, true, false, false, true>;
-                else t.fn = k_wf_trace_w<2, 1, 8, 4, 16, 9, false, false, true, false, false, true>;
-            }
-        }
-    } else {
-        t.name = "k_wf_trace";
-        if (instanced) t.fn = k_wf_trace<8, 8, 2, 32, true, true, 6, true>;
-        else if (spheres) t.fn = k_wf_trace<8, 8, 2, 32, true, true, 6>;
-        else if (scene->bvhDepth > 32) t.fn = k_wf_trace<12, 8, 4, 32, true, false, 8>;
-        else t.fn = k_wf_trace<12, 8, 4, 32, false, false, 8>;
-    }
-    if (t.name[10] == 'p') {   // k_wf_trace_plain: one thread per list entry, no stack in shared memory
-        *out = t;
-        return PB2_OK;
-    }
+    int sceneBits = scene->d.spheres ? TRACE_SPHERES : 0;
+    if (instanced) sceneBits |= TRACE_SPHERES | TRACE_INST;   // an instanced kernel compiles the sphere code as well
+    if (flags & PB2_FLAG_COUNT_TRAVERSAL) return {TK_COUNT, 0};
+    if ((flags & PB2_FLAG_PLAIN_TRACE) || (!records && !linearFits)) return {TK_PLAIN, 0};
+    // alpha masks: the two-child kernel with the alpha test, whatever the other flags
+    if (scene->d.hasAlpha) return records ? TraceKey{TK_WIDE2, sceneBits | TRACE_ALPHA} : TraceKey{TK_PLAIN, 0};
+    // the spheres tuning always has the local-memory spill
+    if (!records) return {TK_LINEAR, sceneBits | (sceneBits || scene->bvhDepth > 32 ? TRACE_DEEP : 0)};
+    if ((flags & PB2_FLAG_POOL) && !sceneBits) return {TK_POOL, 0};
+    const bool ld128 = (flags & PB2_FLAG_LD128) != 0;
+    int features = sceneBits | (ld128 ? TRACE_LD128 : 0) | ((flags & PB2_FLAG_SMALL_STACK) ? TRACE_SMALL_STACK : 0);
+    if (flags & PB2_FLAG_WIDE4) return {TK_WIDE4, features};
+    // the two-child kernel with 32-byte loads: LEAF_TMA on a triangle scene overrides SMALL_STACK; CHAIN in a render unless
+    // SMALL_STACK or LEAF_TMA is set
+    if (!ld128 && (flags & PB2_FLAG_LEAF_TMA) && !sceneBits) features = TRACE_LEAF_TMA;
+    if (!ld128 && render && (flags & PB2_FLAG_CHAIN) && !(flags & (PB2_FLAG_SMALL_STACK | PB2_FLAG_LEAF_TMA))) features |= TRACE_CHAIN;
+    return {TK_WIDE2, features};
+}
+
+// steps: the render's other kernels, for the PB2_VERBOSE line.
+static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool render = false, const char *steps = "") {
+    static const TraceKernelEntry kernels[] = {
+        {TK_COUNT, 0, k_wf_trace_plain<true>, "k_wf_trace_plain<count>", 0},
+        {TK_PLAIN, 0, k_wf_trace_plain<false>, "k_wf_trace_plain", 0},
+        {TK_POOL, 0, k_wf_trace_pool, "k_wf_trace_pool", 4 * sizeof(PoolWarp)},
+        wideTrace<2, 0>(), wideTrace<2, TRACE_SMALL_STACK>(),
+        wideTrace<2, TRACE_LD128>(), wideTrace<2, TRACE_LD128 | TRACE_SMALL_STACK>(),
+        wideTrace<2, TRACE_SPHERES>(), wideTrace<2, TRACE_SPHERES | TRACE_SMALL_STACK>(),
+        wideTrace<2, TRACE_SPHERES | TRACE_LD128>(), wideTrace<2, TRACE_SPHERES | TRACE_LD128 | TRACE_SMALL_STACK>(),
+        wideTrace<2, TRACE_SPHERES | TRACE_INST>(), wideTrace<2, TRACE_SPHERES | TRACE_INST | TRACE_SMALL_STACK>(),
+        wideTrace<2, TRACE_SPHERES | TRACE_INST | TRACE_LD128>(), wideTrace<2, TRACE_SPHERES | TRACE_INST | TRACE_LD128 | TRACE_SMALL_STACK>(),
+        wideTrace<2, TRACE_LEAF_TMA>(),
+        wideTrace<2, TRACE_CHAIN>(), wideTrace<2, TRACE_SPHERES | TRACE_CHAIN>(), wideTrace<2, TRACE_SPHERES | TRACE_INST | TRACE_CHAIN>(),
+        wideTrace<2, TRACE_ALPHA>(), wideTrace<2, TRACE_SPHERES | TRACE_ALPHA>(), wideTrace<2, TRACE_SPHERES | TRACE_INST | TRACE_ALPHA>(),
+        wideTrace<4, 0>(), wideTrace<4, TRACE_SMALL_STACK>(),
+        wideTrace<4, TRACE_LD128>(), wideTrace<4, TRACE_LD128 | TRACE_SMALL_STACK>(),
+        wideTrace<4, TRACE_SPHERES>(), wideTrace<4, TRACE_SPHERES | TRACE_SMALL_STACK>(),
+        wideTrace<4, TRACE_SPHERES | TRACE_LD128>(), wideTrace<4, TRACE_SPHERES | TRACE_LD128 | TRACE_SMALL_STACK>(),
+        wideTrace<4, TRACE_SPHERES | TRACE_INST>(), wideTrace<4, TRACE_SPHERES | TRACE_INST | TRACE_SMALL_STACK>(),
+        wideTrace<4, TRACE_SPHERES | TRACE_INST | TRACE_LD128>(), wideTrace<4, TRACE_SPHERES | TRACE_INST | TRACE_LD128 | TRACE_SMALL_STACK>(),
+        linearTrace<0>(), linearTrace<TRACE_DEEP>(),
+        linearTrace<TRACE_SPHERES | TRACE_DEEP>(), linearTrace<TRACE_SPHERES | TRACE_INST | TRACE_DEEP>(),
+    };
+    const TraceKey want = chooseTraceKernel(scene, flags, render);
+    const TraceKernelEntry *k = nullptr;
+    for (const TraceKernelEntry &e : kernels)
+        if (e.form == want.form && e.features == want.features) k = &e;
+    if (!k)
+        return setError(PB2_ERR_CUDA, "no trace kernel of form " + std::to_string(want.form) + " is compiled for the trace features " +
+                                          std::to_string(want.features));
+    TraceLaunch t;
+    t.fn = k->fn;
+    t.smem = k->smem;
+    t.chain = (k->features & TRACE_CHAIN) != 0;
+    t.name = k->name;
+    if (k->form == TK_POOL && !scene->wfSpill)   // per pipeline: up to 8 resident blocks per SM x 4 warps x PL_R slots x PL_SPILL entries
+        CUDA_TRY(cudaMalloc((void **)&scene->wfSpill, (size_t)kMaxPipes * g_numSMs * 8 * 4 * PL_R * PL_SPILL * sizeof(int2)));
+    if (t.smem) CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)t.smem));
     int blocksPerSM = 1;
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocksPerSM, t.fn, t.block, t.smem));
     // the persistent grid: at most 8 blocks per SM (the pool kernel's spill buffer is sized for 8)
@@ -1193,7 +1201,7 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
                 CUDA_TRY(cudaEventRecord(scene->traceEvents[nEvents], st));
             }
             chain.freeQ = WQ_FREE0 + next;
-            trace.fn<<<trace.grid ? trace.grid : blocks128, trace.block, trace.smem, st>>>(scene->d, pool, WQ_TRACE0 + cur, chain);
+            trace.fn<<<trace.grid, trace.block, trace.smem, st>>>(scene->d, pool, WQ_TRACE0 + cur, chain);
             if (timeTrace) {
                 CUDA_TRY(cudaEventRecord(scene->traceEvents[nEvents + 1], st));
                 nEvents += 2;
@@ -2403,7 +2411,7 @@ int pb2_trace_wavefront(pb2_scene *scene, const pb2_ray *rays, const uint8_t *an
         k_wf_debug_fill<<<blocks, 128>>>(pool, dRays, dAny, N);
         WfChain noChain;
         memset(&noChain, 0, sizeof(noChain));
-        trace.fn<<<trace.grid ? trace.grid : blocks, trace.block, trace.smem>>>(scene->d, pool, WQ_TRACE0, noChain);
+        trace.fn<<<trace.grid, trace.block, trace.smem>>>(scene->d, pool, WQ_TRACE0, noChain);
         k_wf_debug_read<<<blocks, 128>>>(scene->d, pool, N, dOut);
         k_wf_debug_lists<<<std::min(blocks, g_numSMs * 8), 128>>>(pool, dOut);
         e = cudaGetLastError();

@@ -324,6 +324,21 @@ __global__ void __launch_bounds__(128) k_wf_gen(const DRenderParams *__restrict_
     }
 }
 
+// Trace feature mask: what an instantiation of k_wf_trace_w or k_wf_trace is compiled for (its template argument T).
+// The scene bits compile a primitive or a test into the leaf step; an instanced kernel compiles the sphere code as well.
+// The variant bits choose among implementations that return the same records.  selectTraceKernel (pb2_cuda.cu) turns a
+// scene and its PB2_FLAG_* into the mask wanted; every instantiation is listed once there.
+enum {
+    TRACE_SPHERES = 1,
+    TRACE_INST = 2,
+    TRACE_ALPHA = 4,            // alpha-masked triangles: a hit on a texel of value 0 is no hit
+    TRACE_LD128 = 8,            // a record as 16-byte loads; clear: pairs of them as one 32-byte load (ldg256)
+    TRACE_SMALL_STACK = 16,     // 4 instead of 16 stack entries per lane in shared memory (the spill path runs)
+    TRACE_LEAF_TMA = 32,        // leaf records staged into shared memory by the TMA unit (triangles, two-child records)
+    TRACE_CHAIN = 64,           // the light step runs inside the trace kernel (WfChain)
+    TRACE_DEEP = 128,           // k_wf_trace: stack entries beyond the 32 in shared memory spill to local memory
+};
+
 // ---------------------------------------------------------------------------------------------
 // Trace kernel, plain form: one thread per listed ray, BVHAccel::Intersect[P] exactly as written in
 // device/pb2_scene.cuh.  Used when PB2_FLAG_COUNT_TRAVERSAL asks for node / primitive counters
@@ -391,22 +406,26 @@ __global__ void __launch_bounds__(128) k_wf_trace_plain(DScene sc, WfPool pool, 
 // Node-visit and primitive-test counts per ray are the reference's; only the interleaving across
 // lanes differs.  Details:
 //   * the traversal stack lives in shared memory, [depth][thread] (conflict-free), not in local
-//     memory, where it competes with node fetches for L1; entries beyond SDEPTH spill to a small local array (DEEP),
-//     or the host picks this kernel only when the BVH depth fits (DEEP = false);
+//     memory, where it competes with node fetches for L1; entries beyond SDEPTH spill to a small local array
+//     (TRACE_DEEP), or the host picks this kernel only when the BVH depth fits;
 //   * the closest hit so far is written straight into the context (it changes ~1.5 times per ray);
-//     only tMax stays in a register -> 59 registers, 8 blocks of 128 threads per SM;
+//     only tMax stays in a register -> 54 registers for triangles, 8 blocks of 128 threads per SM;
 //   * the descend / pop tail of the node step touches one stack slot with selects instead of
 //     diverging into push and pop branches;
 //   * context words are read / written with streaming hints so nodes + leaf records stay in L2.
+// Two tunings: triangles, and spheres (instanced kernels included; always with TRACE_DEEP).
 // ---------------------------------------------------------------------------------------------
-// INST: object instances (TransformedPrimitive).  An instance is a leaf primitive: the lane saves
+// TRACE_INST: object instances (TransformedPrimitive).  An instance is a leaf primitive: the lane saves
 // (tMax, rest of the leaf) in a 3-entry frame on its stack, takes the ray to instance space
 // (Transform::operator()(Ray), transform.h:251-264) and walks the object's BVH with `instBase` as
 // the stack floor; when that walk ends it comes back through the leaf step (F_EXIT), restores the
 // world-space ray from its context and continues with the rest of the leaf - r.tMax = ray.tMax
 // (primitive.cpp:83) if something was hit inside, the saved tMax otherwise.
-template <int LEAF_T, int FETCH_T, int NSUB, int SDEPTH, bool DEEP, bool SPHERES, int MINB, bool INST = false>
-__global__ void __launch_bounds__(128, MINB) k_wf_trace(DScene sc, WfPool pool, int traceQ, WfChain) {
+template <int T>
+__global__ void __launch_bounds__(128, (T & TRACE_SPHERES) ? 6 : 8) k_wf_trace(DScene sc, WfPool pool, int traceQ, WfChain) {
+    // static: for plain constexpr locals that the lambdas below read, nvcc generates other code than for template arguments
+    static constexpr bool SPHERES = (T & TRACE_SPHERES) != 0, INST = (T & TRACE_INST) != 0, DEEP = (T & TRACE_DEEP) != 0;
+    static constexpr int LEAF_T = SPHERES ? 8 : 12, FETCH_T = 8, NSUB = SPHERES ? 2 : 4, SDEPTH = 32;
     __shared__ int sstack[SDEPTH][128];
     int lstack[DEEP ? 64 - SDEPTH : 1];
     const unsigned FULL = 0xffffffffu;
@@ -645,21 +664,27 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(DScene sc, WfPool pool, 
 // dependent fetch per interior node it descends into instead of one per node it touches
 // (82 -> ~41 on the bench scene), and the two slab tests of a step are independent instructions.
 // ---------------------------------------------------------------------------------------------
-// Template parameters: LEAF_T / FETCH_T = lanes that must wait before the warp runs a leaf / fetch step,
-// NSUB = node visits per scheduling round, SDEPTH = stack entries kept in shared memory (deeper ones
-// spill to local memory), MINB = resident blocks per SM asked of the compiler.
 // WIDTH = 2: the two-child records (DScene::wide); WIDTH = 4: the four-child records (DScene::wide4,
 // device/pb2_wide4.cuh) - two levels of the reference's tree per fetch: a visit tests the four
 // grandchildren's boxes, continues with the first entered one in the reference's visiting order and
 // defers the others (up to three stack entries, the next one to visit on top).
-// LEAFTMA (experiment, PB2_FLAG_LEAF_TMA; not the default, DESIGN.md section 3): the leaf records of the lanes that
-// take a leaf step are staged into shared memory by the TMA unit - one cp.async.bulk (UBLKCP) of up to four 48-byte records
-// per lane, completion counted by one mbarrier per warp - and the triangle tests read them from there.
-template <int WIDTH, int LEAF_T, int FETCH_T, int NSUB, int SDEPTH, int MINB, bool SPHERES = false, bool INST = false, bool LD256 = false,
-          bool LEAFTMA = false, bool ALPHA = false, bool CHAIN = false>
-__global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool, int traceQ, WfChain chain) {
+// T: the trace features (TRACE_*).  With TRACE_LEAF_TMA (an experiment, DESIGN.md section 3) the leaf records of the lanes
+// that take a leaf step are staged into shared memory by the TMA unit - one cp.async.bulk (UBLKCP) of up to four 48-byte
+// records per lane, completion counted by one mbarrier per warp - and the triangle tests read them from there.
+// The resident blocks per SM an instantiation asks of the compiler (__launch_bounds__).
+constexpr int traceMinBlocks(int width, int t) {
+    if (width == 4) return (t & TRACE_SPHERES) ? 5 : 7;
+    if (t & TRACE_LEAF_TMA) return 5;
+    return (t & (TRACE_SPHERES | TRACE_ALPHA)) ? 6 : 9;
+}
+template <int WIDTH, int T>
+__global__ void __launch_bounds__(128, traceMinBlocks(WIDTH, T)) k_wf_trace_w(DScene sc, WfPool pool, int traceQ, WfChain chain) {
     static_assert(WIDTH == 2 || WIDTH == 4, "two- or four-child records");
+    static constexpr bool SPHERES = (T & TRACE_SPHERES) != 0, INST = (T & TRACE_INST) != 0, ALPHA = (T & TRACE_ALPHA) != 0;
+    static constexpr bool LD128 = (T & TRACE_LD128) != 0, LEAFTMA = (T & TRACE_LEAF_TMA) != 0, CHAIN = (T & TRACE_CHAIN) != 0;
     static_assert(!LEAFTMA || (!SPHERES && !INST), "the staging experiment covers triangle scenes");
+    // LEAF_T = 1: a warp turns to its leaves as soon as one lane holds one
+    static constexpr int LEAF_T = 1, FETCH_T = 8, NSUB = 4, SDEPTH = (T & TRACE_SMALL_STACK) ? 4 : 16;
     constexpr int STAGED = 4;   // records staged per lane and leaf step (the reference's default maxnodeprims)
     __shared__ alignas(16) float4 sleaf[LEAFTMA ? 128 * 3 * STAGED : 1];
     __shared__ alignas(8) unsigned long long sbar[LEAFTMA ? 4 : 1];
@@ -756,7 +781,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool
                     if (mode == M_NODE && cur >= 0) {
                         const float4 *w = &sc.wide4[8 * (size_t)cur];
                         float4 q0, q1, q2, q3, q4, q5, q6, q7;
-                        if (LD256) {
+                        if (!LD128) {
                             ldg256(w, q0, q1);
                             ldg256(w + 2, q2, q3);
                             ldg256(w + 4, q4, q5);
@@ -795,7 +820,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool
                 } else if (mode == M_NODE && cur >= 0) {
                     const float4 *w = &sc.wide[4 * (size_t)cur];
                     float4 q0, q1, q2, q3;
-                    if (LD256) {
+                    if (!LD128) {
                         ldg256(w, q0, q1);
                         ldg256(w + 2, q2, q3);
                     } else {
@@ -938,7 +963,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool
                     }
                     float t, b0, b1, b2;
                     if (triangleTest(mk3(a.x, a.y, a.z), mk3(b.x, b.y, b.z), mk3(c4.x, c4.y, c4.z), rs, tMax, &t, &b0, &b1, &b2)) {
-                        // alpha-masked meshes (ALPHA instantiations only): a hit on a texel of value 0 is no hit
+                        // alpha-masked meshes (TRACE_ALPHA instantiations only): a hit on a texel of value 0 is no hit
                         if (ALPHA && (pf & LEAF_ALPHA) && alphaRejects(sc, asInt(a.w), b0, b1, b2, any)) continue;
                         if (any) { flags |= F_FOUND; finished = true; break; }
                         if (pf & LEAF_DEGENERATE) continue;
@@ -1049,7 +1074,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool
 // ---------------------------------------------------------------------------------------------
 // Trace kernel with a per-warp POOL of rays (triangle scenes, two-child records; PB2_FLAG_POOL).  k_wf_trace_w binds a ray
 // to a lane for its whole life, so a step runs with the lanes that happen to be in that phase: ~21 of 32 in node steps, ~6 in
-// leaf steps.  Here a warp owns R = 64 rays whose state lives in shared memory (structure of arrays, one column per ray: ray
+// leaf steps.  Here a warp owns PL_RAYS = 48 rays whose state lives in shared memory (structure of arrays, one column per ray: ray
 // constants, tMax, current record, stack pointer, leaf range, flags; the stack of pending far children next to it), and every
 // step the warp picks up to 32 rays THAT ARE IN THE PHASE BEING RUN, loads their state, runs the step in registers and stores
 // what changed.  Per ray the traversal is the one of k_wf_trace_w, operation for operation (same records, same order, same
@@ -1057,20 +1082,22 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_w(DScene sc, WfPool pool
 // Slot flags: bit 0 any-hit, 1 found, 2-4 direction signs, 5-6 / 7-8 / 9-10 kx ky kz, 11 slow (non-finite), 12-13 phase.
 // ---------------------------------------------------------------------------------------------
 enum { PL_EMPTY = 0, PL_NODE = 1, PL_LEAF = 2, PL_DONE = 3, PL_R = 64, PL_SPILL = 64 };   // PL_R: the most slots a warp can have
-template <int R, int SD>
+// PL_SD stack entries per ray in shared memory: with PL_RAYS rays per warp, 25 KB per block, 8 resident blocks per SM
+enum { PL_RAYS = 48, PL_SD = 8 };
 struct PoolWarp {   // one warp's slice of shared memory
-    float f[10][R];        // ox oy oz ix iy iz tMax Sx Sy Sz
-    int i[6][R];           // cur, sp, ctx, flags, leafFirst, leafN
-    int2 stk[SD][R];       // (child reference, tMin bits); deeper entries go to WfPool::spill
-    int list[R];           // slots chosen for the step, in rank order
+    float f[10][PL_RAYS];        // ox oy oz ix iy iz tMax Sx Sy Sz
+    int i[6][PL_RAYS];           // cur, sp, ctx, flags, leafFirst, leafN
+    int2 stk[PL_SD][PL_RAYS];    // (child reference, tMin bits); deeper entries go to WfPool::spill
+    int list[PL_RAYS];           // slots chosen for the step, in rank order
 };
 
-template <int NSUB, int MINB, int LEAF_T = 24, int FILL_T = 24, int R = 64, int PL_SD = 12>
-__global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool pool, int traceQ, WfChain) {
-    static_assert(R > 32 && R <= PL_R, "a warp owns 33 .. 64 slots");
+__global__ void __launch_bounds__(128, 8) k_wf_trace_pool(DScene sc, WfPool pool, int traceQ, WfChain) {
+    static_assert(PL_RAYS > 32 && PL_RAYS <= PL_R, "a warp owns 33 .. 64 slots");
+    // node visits per node step; rays that must hold a leaf before a leaf step, be done or empty before a flush-and-fill step
+    static constexpr int NSUB = 4, LEAF_T = 16, FILL_T = 12;
     extern __shared__ unsigned char poolSmemRaw[];
-    PoolWarp<R, PL_SD> &pw = reinterpret_cast<PoolWarp<R, PL_SD> *>(poolSmemRaw)[threadIdx.x >> 5];
-    const bool second = (threadIdx.x & 31) + 32 < R;   // this lane also looks after slot lane + 32
+    PoolWarp &pw = reinterpret_cast<PoolWarp *>(poolSmemRaw)[threadIdx.x >> 5];
+    const bool second = (threadIdx.x & 31) + 32 < PL_RAYS;   // this lane also looks after slot lane + 32
     const unsigned FULL = 0xffffffffu;
     const int lane = threadIdx.x & 31;
     const unsigned ltMask = (1u << lane) - 1u;
@@ -1087,14 +1114,14 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace_pool(DScene sc, WfPool p
         else spill[(size_t)s * PL_SPILL + (d - PL_SD)] = e;
     };
     while (true) {
-        // ---- census of the 64 slots
+        // ---- census of the slots
         const int fl0 = pw.i[3][lane], fl1 = second ? pw.i[3][lane + 32] : -1;
         const int m0 = (fl0 >> 12) & 3, m1 = second ? ((fl1 >> 12) & 3) : -1;   // -1: no such slot
         const unsigned bN0 = __ballot_sync(FULL, m0 == PL_NODE), bN1 = __ballot_sync(FULL, m1 == PL_NODE);
         const unsigned bL0 = __ballot_sync(FULL, m0 == PL_LEAF), bL1 = __ballot_sync(FULL, m1 == PL_LEAF);
         const unsigned bD0 = __ballot_sync(FULL, m0 == PL_DONE), bD1 = __ballot_sync(FULL, m1 == PL_DONE);
         const int nN = __popc(bN0) + __popc(bN1), nL = __popc(bL0) + __popc(bL1), nD = __popc(bD0) + __popc(bD1);
-        const int nE = R - nN - nL - nD;
+        const int nE = PL_RAYS - nN - nL - nD;
         int phase;
         if (nD + (exhausted ? 0 : nE) >= FILL_T || (nN == 0 && nL == 0 && (nD > 0 || (!exhausted && nE > 0)))) phase = PL_DONE;   // flush + fill
         else if (nL >= LEAF_T || (nL > 0 && nN == 0)) phase = PL_LEAF;
