@@ -475,6 +475,13 @@ typedef struct pb2_wf_hit {
 int pb2_trace_wavefront(pb2_scene *scene, const pb2_ray *rays, const uint8_t *any_hit, int64_t n, int32_t flags,
                         pb2_wf_hit *out);
 
+/* The persistent trace grid's blocks per SM when several wavefront pipelines share the GPU: the most 128-thread blocks of
+ * the trace kernel (trace_regs registers per thread, trace_smem bytes of shared memory per block) that fit one H100 SM
+ * together with one 128-thread block of the largest list kernel (list_regs, list_smem), at most max_blocks.  Registers
+ * are allocated per warp in units of 256 from the SM's 65 536; an SM holds 2048 threads, 32 blocks and 228 KB of shared
+ * memory, of which 1 KB per block is reserved.  Pure arithmetic, no device needed; 0 when not even one block fits. */
+int pb2_trace_blocks_with_reserve(int32_t trace_regs, int32_t trace_smem, int32_t list_regs, int32_t list_smem, int32_t max_blocks);
+
 /* PathIntegrator::Li for explicit (pixel, sample number) pairs, after the NaN/negative/infinite
  * guard of integrator.cpp:294-315: out_rgb gets 3 floats per sample, out_pfilm 2 floats
  * (CameraSample::pFilm).  Parity/debug entry point; HOST pointers. */

@@ -900,6 +900,8 @@ struct TraceLaunch {
     size_t smem = 0;
     int grid = 0;          // SMs x resident blocks: every trace kernel loops over its list
     bool chain = false;    // the kernel advances shadow / MIS rays itself (no k_wf_advance<light> launch)
+    int carveout = 0;      // the shared-memory carve-out set on the kernel (percent)
+    bool reserved = false; // the grid leaves room for a list-kernel block on every SM
     const char *name = "";
 };
 
@@ -958,8 +960,40 @@ static TraceKey chooseTraceKernel(const pb2_scene *scene, int flags, bool render
     return {TK_WIDE2, features};
 }
 
-// steps: the render's other kernels, for the PB2_VERBOSE line.
-static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool render = false, const char *steps = "") {
+// One H100 SM (sm_90): what the trace grid and a list-kernel block share.
+constexpr int kSmRegs = 65536, kSmThreads = 2048, kSmBlocks = 32, kRegUnit = 256;
+constexpr int kSmSmem = 233472, kBlockSmemReserved = 1024;   // 228 KB of shared memory; 1 KB of it per resident block
+
+static int blockRegs(int regsPerThread, int threads) {
+    return (threads + 31) / 32 * ((regsPerThread * 32 + kRegUnit - 1) / kRegUnit * kRegUnit);
+}
+
+// the shared-memory carve-out (percent of kSmSmem) that holds `bytes` of blocks' shared memory
+static int carveoutPercent(size_t bytes) { return (int)std::min<size_t>(100, (bytes * 100 + kSmSmem - 1) / kSmSmem); }
+
+extern "C" int pb2_trace_blocks_with_reserve(int32_t traceRegs, int32_t traceSmem, int32_t listRegs, int32_t listSmem, int32_t maxBlocks) {
+    const int list = blockRegs(listRegs, 128), trace = blockRegs(traceRegs, 128);
+    int n = std::min(maxBlocks, kSmBlocks - 1);
+    while (n > 0 && (n * trace + list > kSmRegs || (n + 1) * 128 > kSmThreads ||
+                     n * (traceSmem + kBlockSmemReserved) + listSmem + kBlockSmemReserved > kSmSmem))
+        --n;
+    return std::max(n, 0);
+}
+
+// The block of the frame's list kernels (gen, light, shade) that the trace grid leaves room for on every SM when
+// several pipelines share the GPU: the largest registers and static shared memory of the three.
+struct ListReserve {
+    int regs = 0;
+    int smem = 0;
+};
+
+// steps: the render's other kernels, for the PB2_VERBOSE line.  reserve (a render with several pipelines): size the
+// persistent grid so that one list-kernel block fits beside it on every SM, and set the carve-out that holds both.  Only
+// a kernel with registers for 8 blocks per SM (the triangle kernels) gives blocks up: on an H100 the instanced kernel, at
+// 6 blocks, lost more than the overlap gained (DESIGN.md section 3).  PB2_TRACE_BLOCKS=n fixes the blocks per SM (at
+// most what the kernel's occupancy allows).
+static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool render = false, const char *steps = "",
+                             const ListReserve *reserve = nullptr) {
     static const TraceKernelEntry kernels[] = {
         {TK_COUNT, 0, k_wf_trace_plain<true>, "k_wf_trace_plain<count>", 0},
         {TK_PLAIN, 0, k_wf_trace_plain<false>, "k_wf_trace_plain", 0},
@@ -998,19 +1032,33 @@ static int selectTraceKernel(pb2_scene *scene, int flags, TraceLaunch *out, bool
         CUDA_TRY(cudaMalloc((void **)&scene->wfSpill, (size_t)kMaxPipes * g_numSMs * 8 * 4 * PL_R * PL_SPILL * sizeof(int2)));
     if (t.smem) CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)t.smem));
     int blocksPerSM = 1;
+    // the occupancy calculator honours the kernel's carve-out preference: ask with all of the shared memory, not with the
+    // carve-out an earlier render set for fewer blocks
+    CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocksPerSM, t.fn, t.block, t.smem));
     // the persistent grid: at most 8 blocks per SM (the pool kernel's spill buffer is sized for 8)
-    blocksPerSM = std::max(1, std::min(blocksPerSM, 8));
-    // ask for exactly the shared-memory carve-out the resident blocks need; the rest stays L1
+    const int maxBlocks = std::max(1, std::min(blocksPerSM, 8));
     cudaFuncAttributes fa;
     CUDA_TRY(cudaFuncGetAttributes(&fa, t.fn));
-    size_t need = (size_t)blocksPerSM * (fa.sharedSizeBytes + t.smem + 1024);
-    int pct = (int)std::min<size_t>(100, (need * 100 + 233471) / 233472);
-    CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    const int traceSmem = (int)(fa.sharedSizeBytes + t.smem);
+    if (maxBlocks < 8) reserve = nullptr;
+    t.reserved = reserve != nullptr;
+    blocksPerSM = reserve ? std::max(1, pb2_trace_blocks_with_reserve(fa.numRegs, traceSmem, reserve->regs, reserve->smem, maxBlocks)) : maxBlocks;
+    // (read at every render, so that one process can compare settings)
+    const int fixedBlocks = envInt("PB2_TRACE_BLOCKS", 0);
+    if (fixedBlocks > 0) blocksPerSM = std::min(fixedBlocks, maxBlocks);
+    // ask for exactly the shared-memory carve-out the resident blocks (and the reserved list block) need; the rest stays L1
+    size_t need = (size_t)blocksPerSM * (traceSmem + kBlockSmemReserved);
+    if (reserve) need += reserve->smem + kBlockSmemReserved;
+    t.carveout = carveoutPercent(need);
+    CUDA_TRY(cudaFuncSetAttribute(t.fn, cudaFuncAttributePreferredSharedMemoryCarveout, t.carveout));
     static const int verbose = envInt("PB2_VERBOSE", 0);
-    if (verbose)
-        fprintf(stderr, "pb2: trace kernel %s: %d regs, %zu B smem, %d blocks/SM, carve-out %d %%, BVH depth %d%s\n", t.name, fa.numRegs,
-                fa.sharedSizeBytes + t.smem, blocksPerSM, pct, scene->bvhDepth, steps);
+    if (verbose) {
+        char room[96] = "";
+        if (reserve) snprintf(room, sizeof(room), " (reserve: one list block of %d regs, %d B smem)", reserve->regs, reserve->smem);
+        fprintf(stderr, "pb2: trace kernel %s: %d regs, %d B smem, %d blocks/SM%s, carve-out %d %%, BVH depth %d%s\n", t.name, fa.numRegs,
+                traceSmem, blocksPerSM, room, t.carveout, scene->bvhDepth, steps);
+    }
     t.grid = g_numSMs * blocksPerSM;
     *out = t;
     return PB2_OK;
@@ -1130,8 +1178,33 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     char steps[96];
     snprintf(steps, sizeof(steps), "; shade features %d: gen %d, light %d, shade %d, tail %d", features, gen.features,
              advLight.features, advShade.features, finish.features);
+    // Two pipelines, each with half of the contexts and its own lists, on two streams: one pipeline's list kernels run on
+    // the SMs beside the other pipeline's trace kernel.  Both draw samples from the one work counter.
+    // Lazily lit scenes share one request list: one pipeline.  On an H100 two are faster than four on the traversal-bound
+    // soup, the shading-bound killeroo scene and the instanced scene alike.  PB2_PIPES fixes the number (1 ... 4).
+    static const int pipesEnv = envInt("PB2_PIPES", 0);
+    const int pipesWanted = std::min((int)kMaxPipes, pipesEnv > 0 ? pipesEnv : 2);
+    const int nPipes = (lazyLights || capacity < 65536) ? 1 : pipesWanted;
+    // With several pipelines and the class-0 shade step the persistent trace grid leaves room for one block of the
+    // largest list kernel on every SM, and every kernel of the frame asks for the same shared-memory carve-out: an SM
+    // changes its L1 / shared-memory split only when it is idle, so a block whose kernel prefers another split waits
+    // until the SM drains.  (The shading-bound frames of the general shade step were slower so on an H100.)
+    const bool share = nPipes > 1 && advShade.features == SHADE_LAMBERT_AREA;
+    ListReserve reserve;
+    if (share) {
+        for (const void *fn : {(const void *)gen.fn, (const void *)advLight.fn, (const void *)advShade.fn}) {
+            cudaFuncAttributes fa;
+            CUDA_TRY(cudaFuncGetAttributes(&fa, fn));
+            reserve.regs = std::max(reserve.regs, fa.numRegs);
+            reserve.smem = std::max(reserve.smem, (int)fa.sharedSizeBytes);
+        }
+    }
     TraceLaunch trace;
-    if ((rc = selectTraceKernel(scene, flags, &trace, true, steps))) return rc;
+    if ((rc = selectTraceKernel(scene, flags, &trace, true, steps, share ? &reserve : nullptr))) return rc;
+    // no reserve: the list kernels keep the driver's choice of carve-out
+    const int listCarveout = trace.reserved ? trace.carveout : (int)cudaSharedmemCarveoutDefault;
+    for (const void *fn : {(const void *)gen.fn, (const void *)advLight.fn, (const void *)advShade.fn, (const void *)finish.fn, (const void *)k_wf_reset})
+        CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, listCarveout));
     // the scene and this frame's parameters as objects in device memory, read by the gen / advance / finish kernels and
     // wfChainLight.  One buffer per scene, and so per device: every device of a group renders its own replica.
     if (!scene->paramBuf) CUDA_TRY(cudaMalloc(&scene->paramBuf, sizeof(DScene) + sizeof(DRenderParams)));
@@ -1153,14 +1226,6 @@ static int renderWavefront(pb2_scene *scene, const DRenderParams &rp, float4 *fi
     const unsigned finishThreshold = ((flags & PB2_FLAG_COUNT_TRAVERSAL) || lazyLights || textured) ? 0u : (unsigned)(g_numSMs * std::max(0, finishPerSM));
     const int finishBlocks = std::max(1, (int)((finishThreshold + 127) / 128));
     static const int syncEvery = std::max(1, envInt("PB2_SYNC_EVERY", 8));
-    // Two pipelines, each with half of the contexts and its own lists, on two streams: the kernels of one fill the SMs
-    // that the other leaves idle at the end of every launch (a persistent trace launch ends with a stretch in which the last
-    // long rays finish while most warps have exited).  Both draw samples from the one work counter.
-    // Lazily lit scenes share one request list: one pipeline.  On an H100 two are faster than four on the traversal-bound
-    // soup, the shading-bound killeroo scene and the instanced scene alike.  PB2_PIPES fixes the number (1 ... 4).
-    static const int pipesEnv = envInt("PB2_PIPES", 0);
-    const int pipesWanted = std::min((int)kMaxPipes, pipesEnv > 0 ? pipesEnv : 2);
-    const int nPipes = (lazyLights || capacity < 65536) ? 1 : pipesWanted;
     cudaStream_t streams[kMaxPipes] = {stream, stream, stream, stream};
     if (nPipes > 1) {
         if (!scene->forkEvent) CUDA_TRY(cudaEventCreateWithFlags(&scene->forkEvent, cudaEventDisableTiming));

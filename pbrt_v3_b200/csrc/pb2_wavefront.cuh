@@ -1372,6 +1372,10 @@ __global__ void __launch_bounds__(128, MINB) k_wf_advance(const DScene *__restri
 // path with the per-lane state machine (traceLane + laneAdvance, the code of k_li_samples / pb2_li_samples), deposits
 // the sample, and the frame is over.  Same functions, same order of operations per path as the wavefront kernels.
 // k_wf_reset (below) empties the list when k_wf_finish has walked it.
+// No block waits for another: the decision is one atomicCAS on WQ_FINISH.  With several pipelines the trace grid can leave
+// room for one list-kernel block per SM, so a launch of any wavefront kernel may be only partly resident beside another
+// pipeline's kernels: none of them (the trace kernels pull rays from an atomic cursor, the list kernels are grid-stride
+// loops) may spin on another block of its own grid.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool wfFinishNow(const DRenderParams &rp, const WfPool &pool, int traceQ, unsigned threshold) {
     const unsigned n = pool.counts[traceQ];
